@@ -28,6 +28,22 @@ void count_launch(int n = 1);
 
 static inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// Number of CTAs of `kern` that are resident on the current device at once:
+// the grid of a persistent kernel.
+template <typename Kernel>
+static inline cudaError_t resident_ctas(Kernel kern, int threads, size_t smem,
+                                        int* ctas) {
+  int dev = 0, sms = 0, per_sm = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess)
+    e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e == cudaSuccess)
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem);
+  if (e == cudaSuccess && per_sm < 1) e = cudaErrorInvalidConfiguration;
+  if (e == cudaSuccess) *ctas = sms * per_sm;
+  return e;
+}
+
 // Streaming (evict-first) 128-bit / 32-bit stores for write-once outputs.
 __device__ __forceinline__ void st_stream(float4* p, const float4& v) {
   __stcs(p, v);

@@ -20,11 +20,18 @@
 //   finish  + b2 + residual, LayerNorm over the quad that holds each row,
 //           column-pair stores
 //
-// The weights stream through a two-slot ring of 25.6 KB stages (one 1-D bulk
-// copy each, in the order the tensor cores consume them: the K-blocks of W1
-// chunk c, then the two K-blocks of W2 that chunk c feeds).
+// The grid is persistent (one CTA per SM), each CTA looping over 128-row
+// tiles.  The weights stream through a two-slot ring of 25.6 KB stages (one
+// 1-D bulk copy each, in the order the tensor cores consume them: the
+// K-blocks of W1 chunk c, then the two K-blocks of W2 that chunk c feeds; the
+// sequence runs on across the CTA's tiles).  Each stage is one full-width
+// wgmma per operand pair and k8 step; a slot is refilled as soon as the MMAs
+// of the stage before have drained (wgmma.wait_group 1), so the tensor cores
+// drain only at the hidden-chunk conversion.  The next tile's X rows are
+// loaded into registers during the last chunk and stored once its GEMM1 has
+// read the current tile.
 // Shared memory: X tile hi / lo (<= 80 KB) | hidden tile hi / lo (80 KB) |
-// weight ring (2 x 25.6 KB) | mbarriers.
+// weight ring (2 x 25.6 KB) | mbarriers | b1, b2, gamma, beta (2.2 KB).
 //
 // Shapes: E <= 80, E % 4 == 0; hidden % 80 == 0, hidden <= 320.
 #include "common.cuh"
@@ -45,7 +52,8 @@ constexpr int kMaxHidden = 320;
 constexpr int kWStage = 2 * kHC * kKB * 4;          // >= 2 * pad16(E) * kKB * 4
 constexpr int kXBytes = 2 * kABlock;                // E <= 80: two K-blocks
 constexpr int kHBytes = (kHC / kKB) * kABlock;
-constexpr int kSmem = kXBytes + kHBytes + 2 * kWStage + 16;
+constexpr int kCv = kMaxHidden + 3 * kMaxE;         // b1 | b2 | gamma | beta
+constexpr int kSmem = kXBytes + kHBytes + 2 * kWStage + 16 + kCv * 4;
 
 struct Params {
   const float* x;         // [M][E]
@@ -68,150 +76,44 @@ __device__ __forceinline__ uint32_t a_off(int row, int col) {
          (col & 3) * 4u;
 }
 
+// finish of one tile on the GEMM2 accumulator: + b2 + residual, LayerNorm,
+// column-pair stores; `rbase` is the thread's first row, q = lane % 4.  b2 /
+// gamma / beta come from shared memory (`cv`, zero past E) and the residual
+// loads are issued together from always-valid addresses (see linear_epilogue).
 template <int NP2>
-__global__ void __launch_bounds__(kThreads, 1) ffn_tf32_kernel(const Params p) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  unsigned char* xs = smem;
-  unsigned char* hs = smem + kXBytes;
-  const uint32_t xs_a = smem_u32(xs), hs_a = smem_u32(hs);
-  const uint32_t ws_a = hs_a + kHBytes;
-  const uint32_t bar = ws_a + 2 * kWStage;
-  const int tid = threadIdx.x;
-  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    mbar_init(bar + 8u, 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  const int row0 = blockIdx.x * kTileM;
-  const int per_c = p.n_kb1 + kHC / kKB;   // weight stages per hidden chunk
-  const int total = p.n_hc * per_c;
-  auto issue_w = [&](int i) {
-    if (tid != 0 || i >= total) return;
-    const int c = i / per_c, j = i - c * per_c;
-    const float* src;
-    uint32_t bytes;
-    if (j < p.n_kb1) {
-      src = p.w1p + (size_t)(c * p.n_kb1 + j) * (kWStage / 4);
-      bytes = kWStage;
-    } else {
-      const int kb = c * (kHC / kKB) + (j - p.n_kb1);
-      src = p.w2p + (size_t)kb * (2 * NP2 * kKB);
-      bytes = 2u * NP2 * kKB * 4u;
-    }
-    const uint32_t s = i & 1;
-    mbar_arrive_expect_tx(bar + 8u * s, bytes);
-    bulk_g2s(ws_a + s * kWStage, src, bytes, bar + 8u * s);
-  };
-  issue_w(0);
-  issue_w(1);
-
-  // X tile -> hi / lo images, K-block by K-block (columns >= E are zero)
-  for (int kb = 0; kb < p.n_kb1; ++kb) {
-#pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      const int idx = tid + kThreads * i;
-      const int r = idx / kChunks, ch = idx - r * kChunks;
-      const int g = row0 + r, col = kb * kKB + 4 * ch;
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (g < p.M && col < p.E)
-        v = __ldg(reinterpret_cast<const float4*>(p.x + (size_t)g * p.ldx + col));
-      float4 hi;
-      hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
-      const float4 lo = make_float4(v.x - hi.x, v.y - hi.y, v.z - hi.z, v.w - hi.w);
-      unsigned char* a = xs + (size_t)kb * kABlock + a_off(r, 4 * ch);
-      *reinterpret_cast<float4*>(a) = hi;
-      *reinterpret_cast<float4*>(a + kAPart) = lo;
-    }
-  }
-  fence_proxy_async();
-  __syncthreads();
-
-  const int rl = wg * 64 + wq * 16 + (lane >> 2);   // tile row of acc[.. + 0 / 1]
-  float acc2[NP2 / 2];
-#pragma unroll
-  for (int i = 0; i < NP2 / 2; ++i) acc2[i] = 0.f;
-  int it = 0;
-  // one weight stage: wait for its bytes, run the warpgroup's wgmma's, then
-  // release the slot to the copy two stages ahead
-  auto finish_stage = [&]() {
-    wgmma_commit();
-    wgmma_wait<0>();
-    __syncthreads();
-    issue_w(it + 2);
-    ++it;
-  };
-  for (int c = 0; c < p.n_hc; ++c) {
-    float acc1[kHC / 2];
-#pragma unroll
-    for (int i = 0; i < kHC / 2; ++i) acc1[i] = 0.f;
-    for (int j = 0; j < p.n_kb1; ++j) {
-      const uint32_t s = it & 1;
-      mbar_wait(bar + 8u * s, (it >> 1) & 1u);
-      const uint32_t a_hi = xs_a + j * kABlock + wg * 1024u;
-      const uint32_t w_hi = ws_a + s * kWStage;
-      wgmma_fence();
-      wg_kblock_3xtf32<kHC>(acc1, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
-                            w_hi + kHC * kKB * 4, kHC * 16);
-      finish_stage();
-    }
-    acc_fence(acc1);
-    // hidden chunk: + b1, ReLU, hi / lo split -> this warpgroup's rows of hs
-#pragma unroll
-    for (int J = 0; J < kHC / 8; ++J) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int col = 8 * J + 2 * q + e;
-          float v = acc1[4 * J + 2 * h + e];
-          if (p.b1) v += __ldg(p.b1 + c * kHC + col);
-          v = fmaxf(v, 0.f);
-          const float hi = tf32_hi(v);
-          unsigned char* a = hs + (size_t)(col / kKB) * kABlock + a_off(rl + 8 * h, col % kKB);
-          *reinterpret_cast<float*>(a) = hi;
-          *reinterpret_cast<float*>(a + kAPart) = v - hi;
-        }
-      }
-    }
-    fence_proxy_async();
-    __syncthreads();
-    for (int j = 0; j < kHC / kKB; ++j) {
-      const uint32_t s = it & 1;
-      mbar_wait(bar + 8u * s, (it >> 1) & 1u);
-      const uint32_t a_hi = hs_a + j * kABlock + wg * 1024u;
-      const uint32_t w_hi = ws_a + s * kWStage;
-      wgmma_fence();
-      wg_kblock_3xtf32<NP2>(acc2, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
-                            w_hi + NP2 * kKB * 4, NP2 * 16);
-      finish_stage();
-    }
-  }
-  acc_fence(acc2);
-
-  // finish: + b2 + residual, LayerNorm, stores
+__device__ __forceinline__ void ffn_finish(const Params& p, const float (&acc2)[NP2 / 2],
+                                           const float* cv, int rbase, int q) {
+  const float* b2 = cv + kMaxHidden;
+  const float* gamma = b2 + kMaxE;
+  const float* beta = gamma + kMaxE;
   const int E = p.E;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const int row = row0 + rl + 8 * h;
+    const int row = rbase + 8 * h;
     const bool row_ok = row < p.M;
     float t[NP2 / 4];
+    float2 r[NP2 / 8];
+    if (p.residual) {
+#pragma unroll
+      for (int J = 0; J < NP2 / 8; ++J) {
+        const int col = 8 * J + 2 * q;
+        const float* src = row_ok && col < E ? p.residual + (size_t)row * p.ldr + col
+                                             : p.residual;
+        r[J] = __ldg(reinterpret_cast<const float2*>(src));
+      }
+    }
 #pragma unroll
     for (int J = 0; J < NP2 / 8; ++J) {
       const int col = 8 * J + 2 * q;
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         float u = acc2[4 * J + 2 * h + e];
-        if (p.b2 && col < E) u += __ldg(p.b2 + col + e);
+        if (p.b2) u += b2[col + e];  // columns >= E are neither reduced nor stored
         t[2 * J + e] = u;
       }
-      if (p.residual && row_ok && col < E) {
-        const float2 r =
-            __ldg(reinterpret_cast<const float2*>(p.residual + (size_t)row * p.ldr + col));
-        t[2 * J] += r.x;
-        t[2 * J + 1] += r.y;
+      if (p.residual) {
+        t[2 * J] += r[J].x;
+        t[2 * J + 1] += r[J].y;
       }
     }
     if (p.gamma) {
@@ -238,8 +140,8 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_tf32_kernel(const Params p) {
         if (col < E) {
 #pragma unroll
           for (int e = 0; e < 2; ++e)
-            t[2 * J + e] = fmaf((t[2 * J + e] - mean) * rstd, __ldg(p.gamma + col + e),
-                                __ldg(p.beta + col + e));
+            t[2 * J + e] = fmaf((t[2 * J + e] - mean) * rstd, gamma[col + e],
+                                beta[col + e]);
         }
       }
     }
@@ -254,18 +156,184 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_tf32_kernel(const Params p) {
   }
 }
 
+template <int NP2>
+__global__ void __launch_bounds__(kThreads, 1) ffn_tf32_kernel(const Params p) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  unsigned char* xs = smem;
+  unsigned char* hs = smem + kXBytes;
+  const uint32_t xs_a = smem_u32(xs), hs_a = smem_u32(hs);
+  const uint32_t ws_a = hs_a + kHBytes;
+  const uint32_t bar = ws_a + 2 * kWStage;
+  // b1 | b2 | gamma | beta, zero past hidden / E: read by every tile
+  float* cv = reinterpret_cast<float*>(hs + kHBytes + 2 * kWStage + 16);
+  const int tid = threadIdx.x;
+  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    mbar_init(bar + 8u, 1);
+    fence_mbar_init();
+  }
+  for (int i = tid; i < kCv; i += kThreads) {
+    const int j = i < kMaxHidden ? i : (i - kMaxHidden) % kMaxE;
+    const float* v = i < kMaxHidden ? p.b1
+                     : i < kMaxHidden + kMaxE ? p.b2
+                     : i < kMaxHidden + 2 * kMaxE ? p.gamma : p.beta;
+    const int n = i < kMaxHidden ? p.n_hc * kHC : p.E;
+    cv[i] = v && j < n ? __ldg(v + j) : 0.f;
+  }
+  __syncthreads();
+
+  // tiles blockIdx.x, + gridDim.x, ... (the grid is never larger than the
+  // tile count); the weight stages of all of them form one sequence
+  const int n_tiles = (p.M + kTileM - 1) / kTileM;
+  const int per_c = p.n_kb1 + kHC / kKB;   // weight stages per hidden chunk
+  const int per_tile = p.n_hc * per_c;
+  const int total = ((n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1) * per_tile;
+  auto issue_w = [&](int i) {
+    if (tid != 0 || i >= total) return;
+    const int t = i % per_tile;
+    const int c = t / per_c, j = t - c * per_c;
+    const float* src;
+    uint32_t bytes;
+    if (j < p.n_kb1) {
+      src = p.w1p + (size_t)(c * p.n_kb1 + j) * (kWStage / 4);
+      bytes = kWStage;
+    } else {
+      const int kb = c * (kHC / kKB) + (j - p.n_kb1);
+      src = p.w2p + (size_t)kb * (2 * NP2 * kKB);
+      bytes = 2u * NP2 * kKB * 4u;
+    }
+    const uint32_t s = i & 1;
+    mbar_arrive_expect_tx(bar + 8u * s, bytes);
+    bulk_g2s(ws_a + s * kWStage, src, bytes, bar + 8u * s);
+  };
+  issue_w(0);
+  issue_w(1);
+
+  // X tile -> hi / lo images (columns >= E are zero): loaded into registers,
+  // then stored, so the next tile's loads overlap the current tile's tail
+  float4 xv[kXBytes / kABlock][5];
+  auto load_x = [&](int row0) {
+#pragma unroll
+    for (int kb = 0; kb < kXBytes / kABlock; ++kb)
+#pragma unroll
+      for (int i = 0; i < 5; ++i) {
+        const int idx = tid + kThreads * i;
+        const int r = idx / kChunks, ch = idx - r * kChunks;
+        const int g = row0 + r, col = kb * kKB + 4 * ch;
+        xv[kb][i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (kb < p.n_kb1 && g < p.M && col < p.E)
+          xv[kb][i] = __ldg(reinterpret_cast<const float4*>(p.x + (size_t)g * p.ldx + col));
+      }
+  };
+  auto store_x = [&]() {
+#pragma unroll
+    for (int kb = 0; kb < kXBytes / kABlock; ++kb) {
+      if (kb >= p.n_kb1) break;
+#pragma unroll
+      for (int i = 0; i < 5; ++i) {
+        const int idx = tid + kThreads * i;
+        const int r = idx / kChunks, ch = idx - r * kChunks;
+        const float4 v = xv[kb][i];
+        float4 hi;
+        hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
+        const float4 lo = make_float4(v.x - hi.x, v.y - hi.y, v.z - hi.z, v.w - hi.w);
+        unsigned char* a = xs + (size_t)kb * kABlock + a_off(r, 4 * ch);
+        *reinterpret_cast<float4*>(a) = hi;
+        *reinterpret_cast<float4*>(a + kAPart) = lo;
+      }
+    }
+  };
+  load_x(blockIdx.x * kTileM);
+  store_x();
+  fence_proxy_async();
+  __syncthreads();
+
+  const int rl = wg * 64 + wq * 16 + (lane >> 2);   // tile row of acc[.. + 0 / 1]
+  int it = 0;
+  // after issuing stage `it`'s wgmma's: once stage it - 1's have drained (both
+  // warpgroups), its slot takes stage it + 1 while stage it's MMAs run
+  auto next_stage = [&]() {
+    wgmma_commit();
+    wgmma_wait<1>();
+    __syncthreads();
+    if (it >= 1) issue_w(it + 1);
+    ++it;
+  };
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const int row0 = tile * kTileM;
+    const bool more = tile + (int)gridDim.x < n_tiles;
+    float acc2[NP2 / 2];  // written first by a scale-d = 0 MMA, never zeroed
+    for (int c = 0; c < p.n_hc; ++c) {
+      float acc1[kHC / 2];
+      for (int j = 0; j < p.n_kb1; ++j) {
+        const uint32_t s = it & 1;
+        mbar_wait(bar + 8u * s, (it >> 1) & 1u);
+        const uint32_t a_hi = xs_a + j * kABlock + wg * 1024u;
+        const uint32_t w_hi = ws_a + s * kWStage;
+        wgmma_fence();
+        wg_kblock_3xtf32<kHC>(acc1, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
+                              w_hi + kHC * kKB * 4, kHC * 16, j > 0);
+        next_stage();
+      }
+      wgmma_wait<0>();
+      acc_fence(acc1);
+      // the last chunk's GEMM1 has read the X tile: the next tile's loads start
+      if (c == p.n_hc - 1 && more) load_x(row0 + (int)gridDim.x * kTileM);
+      // hidden chunk: + b1, ReLU, hi / lo split -> this warpgroup's rows of hs
+#pragma unroll
+      for (int J = 0; J < kHC / 8; ++J) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * J + 2 * q + e;
+            float v = acc1[4 * J + 2 * h + e];
+            if (p.b1) v += cv[c * kHC + col];
+            v = fmaxf(v, 0.f);
+            const float hi = tf32_hi(v);
+            unsigned char* a = hs + (size_t)(col / kKB) * kABlock + a_off(rl + 8 * h, col % kKB);
+            *reinterpret_cast<float*>(a) = hi;
+            *reinterpret_cast<float*>(a + kAPart) = v - hi;
+          }
+        }
+      }
+      fence_proxy_async();
+      __syncthreads();
+      for (int j = 0; j < kHC / kKB; ++j) {
+        const uint32_t s = it & 1;
+        mbar_wait(bar + 8u * s, (it >> 1) & 1u);
+        const uint32_t a_hi = hs_a + j * kABlock + wg * 1024u;
+        const uint32_t w_hi = ws_a + s * kWStage;
+        wgmma_fence();
+        wg_kblock_3xtf32<NP2>(acc2, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
+                              w_hi + NP2 * kKB * 4, NP2 * 16, c > 0 || j > 0);
+        next_stage();
+      }
+    }
+    // both warpgroups are past the last GEMM1 (the __syncthreads above)
+    if (more) store_x();
+    wgmma_wait<0>();
+    acc_fence(acc2);
+    ffn_finish<NP2>(p, acc2, cv, row0 + rl, q);
+    fence_proxy_async();
+    __syncthreads();
+  }
+}
+
 static inline int pad16(int n) { return (n + 15) / 16 * 16; }
 
 template <int NP2>
-static int launch(const Params& p, int grid, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
+static int launch(const Params& p, int tiles, cudaStream_t st) {
+  static int resident = 0;  // CTAs that fit on the device at once
+  if (!resident) {
     cudaError_t e = cudaFuncSetAttribute(
         ffn_tf32_kernel<NP2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     if (e != cudaSuccess) return (int)e;
-    attr_set = true;
+    e = resident_ctas(ffn_tf32_kernel<NP2>, kThreads, kSmem, &resident);
+    if (e != cudaSuccess) return (int)e;
   }
-  ffn_tf32_kernel<NP2><<<grid, kThreads, kSmem, st>>>(p);
+  ffn_tf32_kernel<NP2><<<tiles < resident ? tiles : resident, kThreads, kSmem, st>>>(p);
   return launch_status();
 }
 
@@ -310,14 +378,14 @@ FBBEV_API int fbbev_ffn_fwd(const float* x, int64_t ldx, const float* w1_packed,
   p.n_kb1 = (embed + kKB - 1) / kKB;
   p.n_hc = hidden / ffn::kHC;
   p.ldx = ldx; p.ldr = ldr; p.ldy = ldy; p.eps = ln_eps;
-  const int grid = (int)ceil_div64(m, ffn::kTileM);
+  const int tiles = (int)ceil_div64(m, ffn::kTileM);
   cudaStream_t st = as_stream(stream);
   count_launch();
   switch (ffn::pad16(embed)) {
-    case 16: return ffn::launch<16>(p, grid, st);
-    case 32: return ffn::launch<32>(p, grid, st);
-    case 48: return ffn::launch<48>(p, grid, st);
-    case 64: return ffn::launch<64>(p, grid, st);
-    default: return ffn::launch<80>(p, grid, st);
+    case 16: return ffn::launch<16>(p, tiles, st);
+    case 32: return ffn::launch<32>(p, tiles, st);
+    case 48: return ffn::launch<48>(p, tiles, st);
+    case 64: return ffn::launch<64>(p, tiles, st);
+    default: return ffn::launch<80>(p, tiles, st);
   }
 }

@@ -15,17 +15,20 @@
 // product is formed as 3xTF32 (see wg_kblock_3xtf32, wgmma.cuh): three
 // wgmma.mma_async kind tf32 per k8 step into the same fp32 accumulator.
 //
-// Structure: one CTA per 128-row tile, two warpgroups (rows 0-63 / 64-127 of
-// the tile).  Per 40-float K-block: all 256 threads load the X rows (global ->
-// registers, issued before waiting on the tensor cores), split them into hi /
-// lo and store them in the K-major core-matrix layout; one thread starts the
-// 1-D bulk copy (TMA) of the pre-packed weight block of the stage, completion
-// on an mbarrier; each warpgroup then issues its wgmma's asynchronously and
-// moves on to the next K-block's loads.  Two stages.  The epilogue works on the
-// accumulator registers: bias, ReLU, residual, LayerNorm (the four lanes of a
-// quad hold one row: two shuffles per reduction), stores of column pairs
-// (optionally two outputs: a column split, for two Linears that share their
-// input).
+// Structure: a persistent grid (as many CTAs as are resident at once), each
+// CTA looping over 128-row tiles; two warpgroups (rows 0-63 / 64-127 of the
+// tile).  The CTA's work is a sequence of steps, one per (tile, 40-float
+// K-block), through two shared-memory stages.  In step g each warpgroup issues
+// the full-width wgmma's of stage g & 1 (the tile's first with scale-d = 0),
+// then, once step g - 1's MMAs have drained, the CTA refills the other stage
+// for step g + 1 while step g's run: one thread starts the 1-D bulk copy (TMA)
+// of the pre-packed weight block, completion on an mbarrier; all 256 threads
+// split the X rows they loaded one step earlier into hi / lo (K-major
+// core-matrix layout) and issue the global loads of step g + 2.  So the X
+// loads of the next tile are in flight during the MMAs and the epilogue of
+// this one.  The epilogue works on the accumulator registers: bias, ReLU,
+// residual, LayerNorm, stores of column pairs (optionally two outputs: a
+// column split, for two Linears that share their input).
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -88,97 +91,19 @@ struct LinearParams {
   float eps;
 };
 
+// Epilogue of one tile on the accumulator registers: bias, ReLU, residual,
+// LayerNorm (the four lanes of a quad hold one row: two shuffles per
+// reduction), column-pair stores (optionally split over two outputs).  `rbase`
+// is the thread's first row, q = lane % 4.  `cv` holds bias / gamma / beta
+// ([3][NPAD], zero past N) in shared memory, and the residual loads of a row
+// are issued in batches from always-valid addresses: a load that sits in a
+// branch in front of its use costs a full memory round trip per column pair.
 template <int NPAD, bool LN>
-__global__ void __launch_bounds__(kLinThreads, 1)
-    linear_tf32_kernel(const LinearParams p) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  constexpr uint32_t w_part = NPAD * kKB * 4;              // bytes of W_hi
-  constexpr uint32_t stage_bytes = 2u * kAPart + 2u * w_part;
-  const int tid = threadIdx.x;
-  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
-  const uint32_t smem_base = smem_u32(smem);
-  const uint32_t bar = smem_u32(smem + 2 * stage_bytes);   // [2] weight stages
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    mbar_init(bar + 8u, 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  const int row0 = blockIdx.x * kTileM;
-  const int n_kb = p.n_kb;
-  auto issue_w = [&](int kb) {
-    if (tid == 0) {
-      const uint32_t s = kb & 1;
-      mbar_arrive_expect_tx(bar + 8u * s, 2u * w_part);
-      bulk_g2s(smem_base + s * stage_bytes + 2u * kAPart,
-               p.wp + (size_t)kb * (2u * w_part / 4u), 2u * w_part, bar + 8u * s);
-    }
-  };
-  issue_w(0);
-  if (n_kb > 1) issue_w(1);
-
-  float acc[NPAD / 2];
-#pragma unroll
-  for (int i = 0; i < NPAD / 2; ++i) acc[i] = 0.f;
-
-  for (int kb = 0; kb < n_kb; ++kb) {
-    const uint32_t s = kb & 1;
-    // X block kb: 128 rows x 10 chunks of 4 floats, 5 chunks per thread
-    float4 v[5];
-#pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      const int idx = tid + kLinThreads * i;
-      const int r = idx / kChunks, ch = idx - r * kChunks;
-      const int g = row0 + r, col = kb * kKB + 4 * ch;
-      const bool ok = g < p.M && col < p.K;
-      v[i] = ok ? __ldg(reinterpret_cast<const float4*>(p.x + (size_t)g * p.ldx + col))
-                : make_float4(0.f, 0.f, 0.f, 0.f);
-      if (p.x_add && ok) {  // query + query_pos in the loader (one fp32 add, as torch)
-        const float4 a = __ldg(
-            reinterpret_cast<const float4*>(p.x_add + (size_t)g * p.ldxa + col));
-        v[i].x = __fadd_rn(v[i].x, a.x);
-        v[i].y = __fadd_rn(v[i].y, a.y);
-        v[i].z = __fadd_rn(v[i].z, a.z);
-        v[i].w = __fadd_rn(v[i].w, a.w);
-      }
-    }
-    if (kb >= 2) {
-      // stage s was read by the wgmma's of K-block kb - 2 (both warpgroups)
-      wgmma_wait<1>();
-      __syncthreads();
-      issue_w(kb);
-    }
-    unsigned char* a_st = smem + (size_t)s * stage_bytes;
-#pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      const int idx = tid + kLinThreads * i;
-      const int r = idx / kChunks, ch = idx - r * kChunks;
-      const float4 x = v[i];
-      float4 hi, lo;
-      hi.x = tf32_hi(x.x); hi.y = tf32_hi(x.y); hi.z = tf32_hi(x.z); hi.w = tf32_hi(x.w);
-      lo.x = x.x - hi.x; lo.y = x.y - hi.y; lo.z = x.z - hi.z; lo.w = x.w - hi.w;
-      const uint32_t off = (uint32_t)(ch * (kTileM / 8) + (r >> 3)) * 128u + (r & 7) * 16u;
-      *reinterpret_cast<float4*>(a_st + off) = hi;
-      *reinterpret_cast<float4*>(a_st + off + kAPart) = lo;
-    }
-    fence_proxy_async();
-    __syncthreads();
-    mbar_wait(bar + 8u * s, (kb >> 1) & 1u);
-    const uint32_t a_hi = smem_base + s * stage_bytes + wg * 1024u;  // 8 row groups
-    const uint32_t w_hi = smem_base + s * stage_bytes + 2u * kAPart;
-    wgmma_fence();
-    wg_kblock_3xtf32<NPAD>(acc, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
-                           w_hi + w_part, NPAD * 16);
-    wgmma_commit();
-  }
-  wgmma_wait<0>();
-  acc_fence(acc);
-
-  // ================================ epilogue ================================
+__device__ __forceinline__ void linear_epilogue(const LinearParams& p,
+                                                const float (&acc)[NPAD / 2],
+                                                const float* cv, int rbase, int q) {
+  constexpr int kBatch = 8;  // residual column pairs in flight per thread
   const int N = p.N;
-  const int q = lane & 3;
-  const int rbase = row0 + wg * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = rbase + 8 * h;
@@ -190,17 +115,27 @@ __global__ void __launch_bounds__(kLinThreads, 1)
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         float u = acc[4 * J + 2 * h + e];
-        if (col < N) {
-          if (p.bias) u += __ldg(p.bias + col + e);
-          if (p.relu) u = fmaxf(u, 0.f);
-        }
-        t[2 * J + e] = u;
+        if (p.bias) u += cv[col + e];
+        if (p.relu) u = fmaxf(u, 0.f);
+        t[2 * J + e] = u;  // columns >= N are neither reduced nor stored
       }
-      if (p.residual && row_ok && col < N) {
-        const float2 r =
-            __ldg(reinterpret_cast<const float2*>(p.residual + (size_t)row * p.ldr + col));
-        t[2 * J] += r.x;
-        t[2 * J + 1] += r.y;
+    }
+    if (p.residual) {
+#pragma unroll
+      for (int J0 = 0; J0 < NPAD / 8; J0 += kBatch) {
+        float2 r[kBatch];
+#pragma unroll
+        for (int b = 0; b < kBatch && J0 + b < NPAD / 8; ++b) {
+          const int col = 8 * (J0 + b) + 2 * q;
+          const float* src = row_ok && col < N ? p.residual + (size_t)row * p.ldr + col
+                                               : p.residual;
+          r[b] = __ldg(reinterpret_cast<const float2*>(src));
+        }
+#pragma unroll
+        for (int b = 0; b < kBatch && J0 + b < NPAD / 8; ++b) {
+          t[2 * (J0 + b)] += r[b].x;
+          t[2 * (J0 + b) + 1] += r[b].y;
+        }
       }
     }
     if (LN) {
@@ -228,8 +163,8 @@ __global__ void __launch_bounds__(kLinThreads, 1)
         if (col < N) {
 #pragma unroll
           for (int e = 0; e < 2; ++e)
-            t[2 * J + e] = fmaf((t[2 * J + e] - mean) * rstd, __ldg(p.gamma + col + e),
-                                __ldg(p.beta + col + e));
+            t[2 * J + e] = fmaf((t[2 * J + e] - mean) * rstd, cv[NPAD + col + e],
+                                cv[2 * NPAD + col + e]);
         }
       }
     }
@@ -245,39 +180,161 @@ __global__ void __launch_bounds__(kLinThreads, 1)
   }
 }
 
+template <int NPAD, bool LN>
+__global__ void __launch_bounds__(kLinThreads, 1)
+    linear_tf32_kernel(const LinearParams p) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  constexpr uint32_t w_part = NPAD * kKB * 4;              // bytes of W_hi
+  constexpr uint32_t stage_bytes = 2u * kAPart + 2u * w_part;
+  const int tid = threadIdx.x;
+  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
+  const uint32_t smem_base = smem_u32(smem);
+  const uint32_t bar = smem_u32(smem + 2 * stage_bytes);   // [2] weight stages
+  float* cv = reinterpret_cast<float*>(smem + 2 * stage_bytes + 16);  // [3][NPAD]
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    mbar_init(bar + 8u, 1);
+    fence_mbar_init();
+  }
+  for (int i = tid; i < 3 * NPAD; i += kLinThreads) {
+    const int c = i % NPAD;
+    const float* v = i < NPAD ? p.bias : (i < 2 * NPAD ? p.gamma : p.beta);
+    cv[i] = v && c < p.N ? __ldg(v + c) : 0.f;
+  }
+  __syncthreads();
+
+  // The CTA's steps: (tile, K-block) pairs, tiles blockIdx.x, + gridDim.x, ...
+  // (the grid is never larger than the tile count); step g uses stage g & 1.
+  const int n_kb = p.n_kb;
+  const int n_tiles = (p.M + kTileM - 1) / kTileM;
+  const int n_steps = (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x * n_kb + n_kb;
+  auto issue_w = [&](int g) {
+    if (tid == 0 && g < n_steps) {
+      const uint32_t s = g & 1;
+      mbar_arrive_expect_tx(bar + 8u * s, 2u * w_part);
+      bulk_g2s(smem_base + s * stage_bytes + 2u * kAPart,
+               p.wp + (size_t)(g % n_kb) * (2u * w_part / 4u), 2u * w_part, bar + 8u * s);
+    }
+  };
+  // X block of step g: 128 rows x 10 chunks of 4 floats, 5 chunks per thread
+  float4 v[5];
+  auto load_x = [&](int g) {
+    if (g >= n_steps) return;
+    const int kb = g % n_kb;
+    const int row0 = ((int)blockIdx.x + g / n_kb * (int)gridDim.x) * kTileM;
+#pragma unroll
+    for (int i = 0; i < 5; ++i) {
+      const int idx = tid + kLinThreads * i;
+      const int r = idx / kChunks, ch = idx - r * kChunks;
+      const int g_row = row0 + r, col = kb * kKB + 4 * ch;
+      const bool ok = g_row < p.M && col < p.K;
+      v[i] = ok ? __ldg(reinterpret_cast<const float4*>(p.x + (size_t)g_row * p.ldx + col))
+                : make_float4(0.f, 0.f, 0.f, 0.f);
+      if (p.x_add && ok) {  // query + query_pos in the loader (one fp32 add, as torch)
+        const float4 a = __ldg(
+            reinterpret_cast<const float4*>(p.x_add + (size_t)g_row * p.ldxa + col));
+        v[i].x = __fadd_rn(v[i].x, a.x);
+        v[i].y = __fadd_rn(v[i].y, a.y);
+        v[i].z = __fadd_rn(v[i].z, a.z);
+        v[i].w = __fadd_rn(v[i].w, a.w);
+      }
+    }
+  };
+  // hi / lo split of the loaded block into stage g & 1 (K-major core matrices)
+  auto store_x = [&](int g) {
+    if (g >= n_steps) return;
+    unsigned char* a_st = smem + (size_t)(g & 1) * stage_bytes;
+#pragma unroll
+    for (int i = 0; i < 5; ++i) {
+      const int idx = tid + kLinThreads * i;
+      const int r = idx / kChunks, ch = idx - r * kChunks;
+      const float4 x = v[i];
+      float4 hi, lo;
+      hi.x = tf32_hi(x.x); hi.y = tf32_hi(x.y); hi.z = tf32_hi(x.z); hi.w = tf32_hi(x.w);
+      lo.x = x.x - hi.x; lo.y = x.y - hi.y; lo.z = x.z - hi.z; lo.w = x.w - hi.w;
+      const uint32_t off = (uint32_t)(ch * (kTileM / 8) + (r >> 3)) * 128u + (r & 7) * 16u;
+      *reinterpret_cast<float4*>(a_st + off) = hi;
+      *reinterpret_cast<float4*>(a_st + off + kAPart) = lo;
+    }
+  };
+
+  issue_w(0);
+  issue_w(1);
+  load_x(0);
+  store_x(0);
+  load_x(1);
+  fence_proxy_async();
+  __syncthreads();
+
+  float acc[NPAD / 2];  // written first by a scale-d = 0 MMA, never zeroed
+  int kb = 0, tile = blockIdx.x;
+  for (int g = 0; g < n_steps; ++g) {
+    const uint32_t s = g & 1;
+    mbar_wait(bar + 8u * s, (g >> 1) & 1u);
+    const uint32_t a_hi = smem_base + s * stage_bytes + wg * 1024u;  // 8 row groups
+    const uint32_t w_hi = smem_base + s * stage_bytes + 2u * kAPart;
+    wgmma_fence();
+    wg_kblock_3xtf32<NPAD>(acc, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
+                           w_hi + w_part, NPAD * 16, kb > 0);
+    wgmma_commit();
+    // step g - 1's MMAs (both warpgroups) have read stage s ^ 1: refill it
+    // with step g + 1 while step g's MMAs run, and start the loads of g + 2
+    wgmma_wait<1>();
+    __syncthreads();
+    if (g >= 1) issue_w(g + 1);
+    store_x(g + 1);
+    load_x(g + 2);
+    if (kb == n_kb - 1) {
+      wgmma_wait<0>();
+      acc_fence(acc);
+      linear_epilogue<NPAD, LN>(p, acc, cv, tile * kTileM + wg * 64 + wq * 16 + (lane >> 2),
+                                lane & 3);
+      kb = 0;
+      tile += gridDim.x;
+    } else {
+      ++kb;
+    }
+    fence_proxy_async();
+    __syncthreads();
+  }
+  wgmma_wait<0>();  // nothing is pending (the last step ends in an epilogue)
+}
+
 static inline int pad16(int n) { return (n + 15) / 16 * 16; }
 static inline int n_kblocks(int k) { return (k + kKB - 1) / kKB; }
 
 template <int NPAD, bool LN>
-static int launch_linear_t(const LinearParams& p, int grid, cudaStream_t st) {
-  constexpr size_t smem = 2 * (2 * (size_t)kAPart + 2 * (size_t)NPAD * kKB * 4) + 16;
-  static bool attr_set = false;
+static int launch_linear_t(const LinearParams& p, int tiles, cudaStream_t st) {
+  constexpr size_t smem =
+      2 * (2 * (size_t)kAPart + 2 * (size_t)NPAD * kKB * 4) + 16 + 3 * NPAD * 4;
+  static int resident = 0;  // CTAs that fit on the device at once
   auto kern = linear_tf32_kernel<NPAD, LN>;
-  if (!attr_set) {
+  if (!resident) {
     cudaError_t e = cudaFuncSetAttribute(
         kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
-    attr_set = true;
+    e = resident_ctas(kern, kLinThreads, smem, &resident);
+    if (e != cudaSuccess) return (int)e;
   }
-  kern<<<grid, kLinThreads, smem, st>>>(p);
+  kern<<<tiles < resident ? tiles : resident, kLinThreads, smem, st>>>(p);
   return launch_status();
 }
 
 template <bool LN>
-static int launch_linear(const LinearParams& p, int npad, int grid, cudaStream_t st) {
+static int launch_linear(const LinearParams& p, int npad, int tiles, cudaStream_t st) {
   switch (npad) {
-    case 16: return launch_linear_t<16, LN>(p, grid, st);
-    case 32: return launch_linear_t<32, LN>(p, grid, st);
-    case 48: return launch_linear_t<48, LN>(p, grid, st);
-    case 64: return launch_linear_t<64, LN>(p, grid, st);
-    case 80: return launch_linear_t<80, LN>(p, grid, st);
-    case 96: return launch_linear_t<96, LN>(p, grid, st);
-    case 112: return launch_linear_t<112, LN>(p, grid, st);
-    case 128: return launch_linear_t<128, LN>(p, grid, st);
-    case 144: return launch_linear_t<144, LN>(p, grid, st);
-    case 160: return launch_linear_t<160, LN>(p, grid, st);
-    case 176: return launch_linear_t<176, LN>(p, grid, st);
-    case 192: return launch_linear_t<192, LN>(p, grid, st);
+    case 16: return launch_linear_t<16, LN>(p, tiles, st);
+    case 32: return launch_linear_t<32, LN>(p, tiles, st);
+    case 48: return launch_linear_t<48, LN>(p, tiles, st);
+    case 64: return launch_linear_t<64, LN>(p, tiles, st);
+    case 80: return launch_linear_t<80, LN>(p, tiles, st);
+    case 96: return launch_linear_t<96, LN>(p, tiles, st);
+    case 112: return launch_linear_t<112, LN>(p, tiles, st);
+    case 128: return launch_linear_t<128, LN>(p, tiles, st);
+    case 144: return launch_linear_t<144, LN>(p, tiles, st);
+    case 160: return launch_linear_t<160, LN>(p, tiles, st);
+    case 176: return launch_linear_t<176, LN>(p, tiles, st);
+    case 192: return launch_linear_t<192, LN>(p, tiles, st);
     default: return FBBEV_ERR_UNSUPPORTED;
   }
 }
@@ -338,11 +395,11 @@ static int linear_run(const float* x, int64_t ldx, const float* x_add,
   p.ldx = ldx; p.ldr = ldr; p.ldy = ldy;
   const bool ln = ln_weight != nullptr;
   if (ln && n > kMaxLnN) return FBBEV_ERR_UNSUPPORTED;
-  const int grid = (int)ceil_div64(m, kTileM);
+  const int tiles = (int)ceil_div64(m, kTileM);
   cudaStream_t st = as_stream(stream);
   count_launch();
-  return ln ? launch_linear<true>(p, pad16(n), grid, st)
-            : launch_linear<false>(p, pad16(n), grid, st);
+  return ln ? launch_linear<true>(p, pad16(n), tiles, st)
+            : launch_linear<false>(p, pad16(n), tiles, st);
 }
 
 FBBEV_API int fbbev_linear_fwd(const float* x, int64_t ldx, const float* packed,
