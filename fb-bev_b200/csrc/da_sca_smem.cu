@@ -118,19 +118,14 @@ template <bool SMEM>
 __device__ __forceinline__ void sample_map(const float* map, int H, int W,
                                            float h_im, float w_im, float wgt,
                                            float (&acc)[kCH]) {
-  if (!(h_im > -1.f && w_im > -1.f && h_im < (float)H && w_im < (float)W))
-    return;
-  const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
-  const float lh = h_im - (float)h_low, lw = w_im - (float)w_low;
-  const float hh = 1.f - lh, hw = 1.f - lw;
-  const bool t = h_low >= 0, btm = h_low + 1 <= H - 1;
-  const bool l = w_low >= 0, r = w_low + 1 <= W - 1;
+  if (!in_image(h_im, w_im, H, W)) return;
+  const Bilinear bl(h_im, w_im);
   // absent corners weigh 0 and read the (always valid) clamped address instead
   // of branching
-  const float w1 = (t && l) ? hh * hw : 0.f, w2 = (t && r) ? hh * lw : 0.f;
-  const float w3 = (btm && l) ? lh * hw : 0.f, w4 = (btm && r) ? lh * lw : 0.f;
-  const int h0 = max(h_low, 0), h1 = min(h_low + 1, H - 1);
-  const int x0 = max(w_low, 0), x1 = min(w_low + 1, W - 1);
+  const float w1 = bl.ok1(H, W) ? bl.w1 : 0.f, w2 = bl.ok2(H, W) ? bl.w2 : 0.f;
+  const float w3 = bl.ok3(H, W) ? bl.w3 : 0.f, w4 = bl.ok4(H, W) ? bl.w4 : 0.f;
+  const int h0 = max(bl.h_low, 0), h1 = min(bl.h_low + 1, H - 1);
+  const int x0 = max(bl.w_low, 0), x1 = min(bl.w_low + 1, W - 1);
   const float* p1 = map + (h0 * W + x0) * kE;
   const float* p2 = map + (h0 * W + x1) * kE;
   const float* p3 = map + (h1 * W + x0) * kE;
@@ -193,12 +188,11 @@ __device__ __forceinline__ void sca_pass(const ScaSmemParams& P, const ScaCtx& C
     for (int i = 0; i < 4; ++i) off4[i] = __ldg(o4 + i);
     // depth weight of anchor z = m & 3, shared out below (:196-199, :584-591)
     const int z = m & 3;
-    const float d = __ldg(P.ref_depth + rb + z);
-    float fb = floorf(__fdiv_rn(__fsub_rn(d, P.d_min), P.d_step));
-    fb = fminf(fmaxf(fb, 0.f), (float)(P.DC - 1));
+    const int bin =
+        depth_bin(__ldg(P.ref_depth + rb + z), P.d_min, P.d_step, P.DC);
     const float2 rz = z == 0 ? rxy[0] : z == 1 ? rxy[1] : z == 2 ? rxy[2]
                                                                  : rxy[3];
-    dwz = sample_scalar(C.dp + (int)fb, C.H, C.W, P.DC, pix(rz.y, C.H),
+    dwz = sample_scalar(C.dp + bin, C.H, C.W, P.DC, pix(rz.y, C.H),
                         pix(rz.x, C.W));
     // softmax over the head's 8 logits (:540)
     w[0] = la.x; w[1] = la.y; w[2] = la.z; w[3] = la.w;

@@ -18,89 +18,30 @@ namespace fbbev {
 
 constexpr int kMsdaBwdThreads = 128;
 
+// CH > 0: the head's CH channels of grad_out in registers, the channel loop
+// unrolled.  CH == 0: any head width, ch channels walked serially, grad_out
+// read per channel.
 template <int CH, bool kDet>
 __global__ void __launch_bounds__(kMsdaBwdThreads) msda_bwd_kernel(
     const float* __restrict__ value, const int64_t* __restrict__ shapes,
     const int64_t* __restrict__ lstart, const float* __restrict__ loc,
     const float* __restrict__ attw, const float* __restrict__ grad_out,
-    int64_t n_items, int n_value, int heads, int levels, int nq, int points,
-    float* __restrict__ grad_value, float* __restrict__ grad_loc,
-    float* __restrict__ grad_attw, DetSink det) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n_items) return;
-  const int m = (int)(idx % heads);
-  const int64_t bq = idx / heads;
-  const int b = (int)(bq / nq);
-  const int E = heads * CH;
-  float go[CH];
-#pragma unroll
-  for (int c = 0; c < CH; ++c) go[c] = __ldg(grad_out + bq * E + m * CH + c);
-  const int64_t wbase = idx * levels * points;
-  int pcell = 0;  // kDet: padded cells of the levels before l
-  for (int l = 0; l < levels; ++l) {
-    const int H = (int)__ldg(shapes + 2 * l), W = (int)__ldg(shapes + 2 * l + 1);
-    const int64_t voff = ((int64_t)b * n_value + __ldg(lstart + l)) * E + m * CH;
-    const float* val = value + voff;
-    float* gval = grad_value + voff;
-    for (int p = 0; p < points; ++p) {
-      const int64_t wi = wbase + (int64_t)l * points + p;
-      const float2 xy = __ldg(reinterpret_cast<const float2*>(loc) + wi);
-      const float wgt = __ldg(attw + wi);
-      const float h = __fsub_rn(__fmul_rn(xy.y, (float)H), 0.5f);
-      const float w = __fsub_rn(__fmul_rn(xy.x, (float)W), 0.5f);
-      if (!(h > -1.f && w > -1.f && h < (float)H && w < (float)W)) continue;
-      if (kDet) {
-        det.key[wi] = det_value_key(h, w, W, pcell, heads, m);
-        det.rec[wi] = make_float3(h, w, wgt);
-      }
-      const int h_low = (int)floorf(h), w_low = (int)floorf(w);
-      const int h_high = h_low + 1, w_high = w_low + 1;
-      const float lh = h - (float)h_low, lw = w - (float)w_low;
-      const float hh = 1.f - lh, hw = 1.f - lw;
-      const float w1 = hh * hw, w2 = hh * lw, w3 = lh * hw, w4 = lh * lw;
-      const bool ok1 = h_low >= 0 && w_low >= 0;
-      const bool ok2 = h_low >= 0 && w_high <= W - 1;
-      const bool ok3 = h_high <= H - 1 && w_low >= 0;
-      const bool ok4 = h_high <= H - 1 && w_high <= W - 1;
-      const int64_t o1 = ((int64_t)h_low * W + w_low) * E;
-      const int64_t o2 = o1 + E, o3 = o1 + (int64_t)W * E, o4 = o3 + E;
-      float g_h = 0.f, g_w = 0.f, g_a = 0.f;
-#pragma unroll
-      for (int c = 0; c < CH; ++c) {
-        const float top = go[c] * wgt;
-        float v1 = 0.f, v2 = 0.f, v3 = 0.f, v4 = 0.f;
-        if (ok1) { v1 = __ldg(val + o1 + c); if (!kDet) atomicAdd(gval + o1 + c, w1 * top); }
-        if (ok2) { v2 = __ldg(val + o2 + c); if (!kDet) atomicAdd(gval + o2 + c, w2 * top); }
-        if (ok3) { v3 = __ldg(val + o3 + c); if (!kDet) atomicAdd(gval + o3 + c, w3 * top); }
-        if (ok4) { v4 = __ldg(val + o4 + c); if (!kDet) atomicAdd(gval + o4 + c, w4 * top); }
-        g_h += (-hw * v1 - lw * v2 + hw * v3 + lw * v4) * top;
-        g_w += (-hh * v1 + hh * v2 - lh * v3 + lh * v4) * top;
-        g_a += (w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4) * go[c];
-      }
-      grad_attw[wi] = g_a;
-      reinterpret_cast<float2*>(grad_loc)[wi] =
-          make_float2((float)W * g_w, (float)H * g_h);
-    }
-    pcell += (H + 1) * (W + 1);
-  }
-}
-
-// Any head width: one thread per (batch, query, head), channels walked serially.
-template <bool kDet>
-__global__ void __launch_bounds__(kMsdaBwdThreads) msda_bwd_generic_kernel(
-    const float* __restrict__ value, const int64_t* __restrict__ shapes,
-    const int64_t* __restrict__ lstart, const float* __restrict__ loc,
-    const float* __restrict__ attw, const float* __restrict__ grad_out,
-    int64_t n_items, int n_value, int heads, int ch, int levels, int nq,
+    int64_t n_items, int n_value, int heads, int ch_rt, int levels, int nq,
     int points, float* __restrict__ grad_value, float* __restrict__ grad_loc,
     float* __restrict__ grad_attw, DetSink det) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n_items) return;
+  const int ch = CH > 0 ? CH : ch_rt;
   const int m = (int)(idx % heads);
   const int64_t bq = idx / heads;
   const int b = (int)(bq / nq);
   const int E = heads * ch;
-  const float* go = grad_out + bq * E + m * ch;
+  const float* gptr = grad_out + bq * E + m * ch;
+  float go[CH > 0 ? CH : 1];
+  if (CH > 0) {
+#pragma unroll
+    for (int c = 0; c < CH; ++c) go[c] = __ldg(gptr + c);
+  }
   const int64_t wbase = idx * levels * points;
   int pcell = 0;  // kDet: padded cells of the levels before l
   for (int l = 0; l < levels; ++l) {
@@ -112,36 +53,26 @@ __global__ void __launch_bounds__(kMsdaBwdThreads) msda_bwd_generic_kernel(
       const int64_t wi = wbase + (int64_t)l * points + p;
       const float2 xy = __ldg(reinterpret_cast<const float2*>(loc) + wi);
       const float wgt = __ldg(attw + wi);
-      const float h = __fsub_rn(__fmul_rn(xy.y, (float)H), 0.5f);
-      const float w = __fsub_rn(__fmul_rn(xy.x, (float)W), 0.5f);
-      if (!(h > -1.f && w > -1.f && h < (float)H && w < (float)W)) continue;
-      if (kDet) {
-        det.key[wi] = det_value_key(h, w, W, pcell, heads, m);
-        det.rec[wi] = make_float3(h, w, wgt);
-      }
-      const int h_low = (int)floorf(h), w_low = (int)floorf(w);
-      const int h_high = h_low + 1, w_high = w_low + 1;
-      const float lh = h - (float)h_low, lw = w - (float)w_low;
-      const float hh = 1.f - lh, hw = 1.f - lw;
-      const float w1 = hh * hw, w2 = hh * lw, w3 = lh * hw, w4 = lh * lw;
-      const bool ok1 = h_low >= 0 && w_low >= 0;
-      const bool ok2 = h_low >= 0 && w_high <= W - 1;
-      const bool ok3 = h_high <= H - 1 && w_low >= 0;
-      const bool ok4 = h_high <= H - 1 && w_high <= W - 1;
-      const int64_t o1 = ((int64_t)h_low * W + w_low) * E;
+      const float h = pix(xy.y, H), w = pix(xy.x, W);
+      if (!in_image(h, w, H, W)) continue;
+      const Bilinear bl(h, w);
+      if (kDet)
+        det.value_record(wi, pcell + bl.padded_cell(W), heads, m, h, w, wgt);
+      const int64_t o1 = bl.offset(W, E);
       const int64_t o2 = o1 + E, o3 = o1 + (int64_t)W * E, o4 = o3 + E;
       float g_h = 0.f, g_w = 0.f, g_a = 0.f;
-      for (int c = 0; c < ch; ++c) {
-        const float g = __ldg(go + c);
+#pragma unroll
+      for (int c = 0; c < (CH > 0 ? CH : ch); ++c) {
+        const float g = CH > 0 ? go[c] : __ldg(gptr + c);
         const float top = g * wgt;
         float v1 = 0.f, v2 = 0.f, v3 = 0.f, v4 = 0.f;
-        if (ok1) { v1 = __ldg(val + o1 + c); if (!kDet) atomicAdd(gval + o1 + c, w1 * top); }
-        if (ok2) { v2 = __ldg(val + o2 + c); if (!kDet) atomicAdd(gval + o2 + c, w2 * top); }
-        if (ok3) { v3 = __ldg(val + o3 + c); if (!kDet) atomicAdd(gval + o3 + c, w3 * top); }
-        if (ok4) { v4 = __ldg(val + o4 + c); if (!kDet) atomicAdd(gval + o4 + c, w4 * top); }
-        g_h += (-hw * v1 - lw * v2 + hw * v3 + lw * v4) * top;
-        g_w += (-hh * v1 + hh * v2 - lh * v3 + lh * v4) * top;
-        g_a += (w1 * v1 + w2 * v2 + w3 * v3 + w4 * v4) * g;
+        if (bl.ok1(H, W)) { v1 = __ldg(val + o1 + c); if (!kDet) atomicAdd(gval + o1 + c, bl.w1 * top); }
+        if (bl.ok2(H, W)) { v2 = __ldg(val + o2 + c); if (!kDet) atomicAdd(gval + o2 + c, bl.w2 * top); }
+        if (bl.ok3(H, W)) { v3 = __ldg(val + o3 + c); if (!kDet) atomicAdd(gval + o3 + c, bl.w3 * top); }
+        if (bl.ok4(H, W)) { v4 = __ldg(val + o4 + c); if (!kDet) atomicAdd(gval + o4 + c, bl.w4 * top); }
+        g_h += (-bl.hw * v1 - bl.lw * v2 + bl.hw * v3 + bl.lw * v4) * top;
+        g_w += (-bl.hh * v1 + bl.hh * v2 - bl.lh * v3 + bl.lh * v4) * top;
+        g_a += (bl.w1 * v1 + bl.w2 * v2 + bl.w3 * v3 + bl.w4 * v4) * g;
       }
       grad_attw[wi] = g_a;
       reinterpret_cast<float2*>(grad_loc)[wi] =
@@ -161,28 +92,14 @@ static int launch_msda_bwd(const float* value, const int64_t* spatial_shapes,
                            const DetSink& det, cudaStream_t st) {
   const unsigned grid = (unsigned)ceil_div64(n_items, kMsdaBwdThreads);
   count_launch();
-#define FBBEV_LAUNCH(CHV)                                                     \
-  msda_bwd_kernel<CHV, kDet><<<grid, kMsdaBwdThreads, 0, st>>>(               \
-      value, spatial_shapes, level_start, loc, attw, grad_out, n_items,       \
-      n_value, heads, levels, nq, points, grad_value, grad_loc, grad_attw,    \
-      det);                                                                   \
-  break
-  switch (ch) {
-    case 4: FBBEV_LAUNCH(4);
-    case 8: FBBEV_LAUNCH(8);
-    case 10: FBBEV_LAUNCH(10);
-    case 16: FBBEV_LAUNCH(16);
-    case 20: FBBEV_LAUNCH(20);
-    case 32: FBBEV_LAUNCH(32);
-    case 64: FBBEV_LAUNCH(64);
-    default:
-      msda_bwd_generic_kernel<kDet><<<grid, kMsdaBwdThreads, 0, st>>>(
-          value, spatial_shapes, level_start, loc, attw, grad_out, n_items,
-          n_value, heads, ch, levels, nq, points, grad_value, grad_loc,
-          grad_attw, det);
-      break;
-  }
-#undef FBBEV_LAUNCH
+  auto launch = [&](auto CH) {
+    msda_bwd_kernel<CH.value, kDet><<<grid, kMsdaBwdThreads, 0, st>>>(
+        value, spatial_shapes, level_start, loc, attw, grad_out, n_items,
+        n_value, heads, ch, levels, nq, points, grad_value, grad_loc,
+        grad_attw, det);
+  };
+  if (!dispatch(HeadWidths(), ch, launch))
+    launch(std::integral_constant<int, 0>());
   return launch_status();
 }
 

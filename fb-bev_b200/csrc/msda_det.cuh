@@ -27,33 +27,17 @@ struct DetSink {
                              // (nq, heads*ch) of the pass's sample
   int64_t item0 = 0;         // cross-attention: first (b, q, head) item
   int cam = 0;               // cross-attention: camera of the pass
+
+  // value-gradient record r of an in-image sample of head m; `cell` is the
+  // sample's padded cell (Bilinear::padded_cell) plus the padded cells of the
+  // levels before its own, the key head-minor
+  __device__ __forceinline__ void value_record(int64_t r, int cell, int heads,
+                                               int m, float h_im, float w_im,
+                                               float coef) const {
+    key[r] = (uint32_t)(cell * heads + m);
+    rec[r] = make_float3(h_im, w_im, coef);
+  }
 };
-
-// In-image test of a bilinear sample (sample_bwd / scatter_scalar's test)
-__device__ __forceinline__ bool det_in_image(float h_im, float w_im, int H,
-                                             int W) {
-  return h_im > -1.f && w_im > -1.f && h_im < (float)H && w_im < (float)W;
-}
-
-// Top-left corner cell of an in-image sample in the (H+1) x (W+1) grid padded
-// by one row and column before the image (h_low, w_low >= -1)
-__device__ __forceinline__ int det_cell(float h_im, float w_im, int W) {
-  return ((int)floorf(h_im) + 1) * (W + 1) + (int)floorf(w_im) + 1;
-}
-
-// value-gradient key: cell of level l (pcell = padded cells of the levels
-// before l), head-minor
-__device__ __forceinline__ uint32_t det_value_key(float h_im, float w_im,
-                                                  int W, int pcell, int heads,
-                                                  int m) {
-  return (uint32_t)((pcell + det_cell(h_im, w_im, W)) * heads + m);
-}
-
-// Head widths of the fused kernels (FBBEV_CH_DISPATCH)
-static inline bool fused_head_width(int ch) {
-  return ch == 4 || ch == 8 || ch == 10 || ch == 16 || ch == 20 || ch == 32 ||
-         ch == 64;
-}
 
 // One record pass of the backward kernels (launchers in msda_fused_bwd.cu and
 // msda_bwd.cu).  Pointers are those of the pass's sample; the cross-attention

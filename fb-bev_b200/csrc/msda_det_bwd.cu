@@ -147,14 +147,9 @@ __global__ void cell_range_kernel(const uint32_t* __restrict__ sk, int64_t n,
 }
 
 // ---------------- gather ----------------------------------------------------
-// bilinear weight of corner k = 2 * dy + dx of a sample, the twin's arithmetic
-__device__ __forceinline__ float corner_weight(float h_im, float w_im, int k) {
-  const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
-  const float lh = h_im - (float)h_low, lw = w_im - (float)w_low;
-  const float hh = 1.f - lh, hw = 1.f - lw;
-  return k == 0 ? hh * hw : k == 1 ? hh * lw : k == 2 ? lh * hw : lh * lw;
-}
-
+// The weight of corner k = 2 * dy + dx of a record is Bilinear's, as in the
+// twin kernel that wrote the record.
+//
 // grad_value of one (n_value, heads, ch) map.  Record r belongs to grad row
 // r / LP of G (nq, heads*ch).  kFusedArith: the product (a * w) * g of
 // sample_bwd (msda_fused_bwd.cu); otherwise w * (g * a) of msda_bwd.cu.
@@ -186,7 +181,7 @@ __global__ void __launch_bounds__(kGatherThreads) gather_value_kernel(
     for (int j = rg.x; j < rg.y; ++j) {
       const uint32_t r = __ldg(order + j);
       const float3 R = rec[r];
-      const float wk = corner_weight(R.x, R.y, k);
+      const float wk = Bilinear(R.x, R.y).weight(k);
       const float g = __ldg(G + (int64_t)(r / LP) * ch + c);
       acc = __fadd_rn(acc, kFusedArith ? __fmul_rn(__fmul_rn(R.z, wk), g)
                                        : __fmul_rn(wk, __fmul_rn(g, R.z)));
@@ -216,7 +211,8 @@ __global__ void __launch_bounds__(kGatherThreads) gather_depth_kernel(
                         (k & 1)) * DC + d];
     for (int j = rg.x; j < rg.y; ++j) {
       const float3 R = rec[__ldg(order + j)];
-      acc = __fadd_rn(acc, __fmul_rn(corner_weight(R.x, R.y, k), R.z));
+      acc = __fadd_rn(acc,
+                      __fmul_rn(Bilinear(R.x, R.y).weight(k), R.z));
     }
   }
   gdp[(int64_t)b * n_cams * per_cam + idx] = acc;
@@ -484,8 +480,7 @@ FBBEV_API int fbbev_da_sca_bwd_det(
       ch <= 0 || levels <= 0 || points <= 0 || Z <= 0 || DC <= 0 ||
       !dbound_host || points % Z != 0)
     return FBBEV_ERR_INVALID_ARGUMENT;
-  if (!fused_head_width(ch) || !(Z == 1 || Z == 2 || Z == 4 || Z == 8))
-    return FBBEV_ERR_UNSUPPORTED;
+  if (!fused_head_width(ch) || !fused_z(Z)) return FBBEV_ERR_UNSUPPORTED;
   if ((int64_t)bs * nq == 0) return FBBEV_OK;
   if (!value || !depth_prob || !ref_cam || !ref_depth || !mask || !offsets ||
       !logits || !spatial_shapes || !level_start || !grad_out ||
@@ -498,11 +493,8 @@ FBBEV_API int fbbev_da_sca_bwd_det(
     const int rc = check_workspace(L, workspace, workspace_bytes);
     if (rc != FBBEV_OK) return rc;
   }
-  DaScaParams P;
-  P.d_min = dbound_host[0];
-  P.d_step = dbound_host[2];
-  P.bs = bs; P.n_cams = n_cams; P.nq = nq; P.n_value = n_value;
-  P.heads = heads; P.levels = levels; P.points = points; P.DC = DC;
+  const DaScaParams P = da_sca_params(dbound_host, bs, n_cams, nq, n_value,
+                                      heads, levels, points, DC);
   cudaStream_t st = as_stream(stream);
   const int E = heads * ch;
   for (int b = 0; b < bs; ++b) {

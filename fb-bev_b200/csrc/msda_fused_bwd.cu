@@ -57,14 +57,14 @@ __device__ __forceinline__ void sample_bwd(const float* __restrict__ val,
                                            const float (&G)[CH], float& S,
                                            float& gh, float& gw) {
   S = gh = gw = 0.f;
-  if (!(h_im > -1.f && w_im > -1.f && h_im < (float)H && w_im < (float)W))
-    return;
+  if (!in_image(h_im, w_im, H, W)) return;
   constexpr int VW = VecWidth<CH>::value;
-  const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
+  const Bilinear bl(h_im, w_im);
+  // corner flags and offsets spelled out from h_low / w_low rather than
+  // okN() / offset(): same values, but ptxas then spills less in the kDet
+  // cross-attention instantiations
+  const int h_low = bl.h_low, w_low = bl.w_low;
   const int h_high = h_low + 1, w_high = w_low + 1;
-  const float lh = h_im - (float)h_low, lw = w_im - (float)w_low;
-  const float hh = 1.f - lh, hw = 1.f - lw;
-  const float w1 = hh * hw, w2 = hh * lw, w3 = lh * hw, w4 = lh * lw;
   const bool ok1 = h_low >= 0 && w_low >= 0;
   const bool ok2 = h_low >= 0 && w_high <= W - 1;
   const bool ok3 = h_high <= H - 1 && w_low >= 0;
@@ -83,15 +83,15 @@ __device__ __forceinline__ void sample_bwd(const float* __restrict__ val,
 #pragma unroll
     for (int k = 0; k < VW; ++k) {
       const float g = G[c + k];
-      S += g * (w1 * v1[k] + w2 * v2[k] + w3 * v3[k] + w4 * v4[k]);
-      gh += g * (-hw * v1[k] - lw * v2[k] + hw * v3[k] + lw * v4[k]);
-      gw += g * (-hh * v1[k] + hh * v2[k] - lh * v3[k] + lh * v4[k]);
+      S += g * (bl.w1 * v1[k] + bl.w2 * v2[k] + bl.w3 * v3[k] + bl.w4 * v4[k]);
+      gh += g * (-bl.hw * v1[k] - bl.lw * v2[k] + bl.hw * v3[k] + bl.lw * v4[k]);
+      gw += g * (-bl.hh * v1[k] + bl.hh * v2[k] - bl.lh * v3[k] + bl.lh * v4[k]);
     }
     if (gval) {
-      if (ok1) red_vec<VW>(gval + o1 + c, a * w1, G + c);
-      if (ok2) red_vec<VW>(gval + o2 + c, a * w2, G + c);
-      if (ok3) red_vec<VW>(gval + o3 + c, a * w3, G + c);
-      if (ok4) red_vec<VW>(gval + o4 + c, a * w4, G + c);
+      if (ok1) red_vec<VW>(gval + o1 + c, a * bl.w1, G + c);
+      if (ok2) red_vec<VW>(gval + o2 + c, a * bl.w2, G + c);
+      if (ok3) red_vec<VW>(gval + o3 + c, a * bl.w3, G + c);
+      if (ok4) red_vec<VW>(gval + o4 + c, a * bl.w4, G + c);
     }
   }
 }
@@ -101,19 +101,13 @@ __device__ __forceinline__ void sample_bwd(const float* __restrict__ val,
 __device__ __forceinline__ void scatter_scalar(float* __restrict__ gmap, int H,
                                                int W, int stride, float h_im,
                                                float w_im, float g) {
-  if (!(h_im > -1.f && w_im > -1.f && h_im < (float)H && w_im < (float)W))
-    return;
-  const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
-  const int h_high = h_low + 1, w_high = w_low + 1;
-  const float lh = h_im - (float)h_low, lw = w_im - (float)w_low;
-  const float hh = 1.f - lh, hw = 1.f - lw;
-  float* p1 = gmap + ((int64_t)h_low * W + w_low) * stride;
-  if (h_low >= 0 && w_low >= 0) atomicAdd(p1, hh * hw * g);
-  if (h_low >= 0 && w_high <= W - 1) atomicAdd(p1 + stride, hh * lw * g);
-  if (h_high <= H - 1 && w_low >= 0)
-    atomicAdd(p1 + (int64_t)W * stride, lh * hw * g);
-  if (h_high <= H - 1 && w_high <= W - 1)
-    atomicAdd(p1 + (int64_t)W * stride + stride, lh * lw * g);
+  if (!in_image(h_im, w_im, H, W)) return;
+  const Bilinear bl(h_im, w_im);
+  float* p1 = gmap + bl.offset(W, stride);
+  if (bl.ok1(H, W)) atomicAdd(p1, bl.w1 * g);
+  if (bl.ok2(H, W)) atomicAdd(p1 + stride, bl.w2 * g);
+  if (bl.ok3(H, W)) atomicAdd(p1 + (int64_t)W * stride, bl.w3 * g);
+  if (bl.ok4(H, W)) atomicAdd(p1 + (int64_t)W * stride + stride, bl.w4 * g);
 }
 
 // G[0..CH) = grad_out of one head, divided by `cnt`
@@ -179,13 +173,12 @@ __global__ void __launch_bounds__(kFusedBwdThreads) msda_fused_bwd_kernel(
       const float wgt = expf(__ldg(logits + wi) - mx) * inv;
       const float h_im = pix(ly, H), w_im = pix(lx, W);
       float S, gh, gw;
-      sample_bwd<CH>(value + voff,
-                     !kDet && grad_value ? grad_value + voff : nullptr, H, W,
-                     E, h_im, w_im, wgt, G, S, gh, gw);
-      if (kDet && det.key && det_in_image(h_im, w_im, H, W)) {
-        det.key[wi] = det_value_key(h_im, w_im, W, pcell, heads, m);
-        det.rec[wi] = make_float3(h_im, w_im, wgt);
-      }
+      sample_bwd<CH>(
+          value + voff, !kDet && grad_value ? grad_value + voff : nullptr, H,
+          W, E, h_im, w_im, wgt, G, S, gh, gw);
+      if (kDet && det.key && in_image(h_im, w_im, H, W))
+        det.value_record(wi, pcell + Bilinear(h_im, w_im).padded_cell(W),
+                         heads, m, h_im, w_im, wgt);
       if (grad_offsets)
         reinterpret_cast<float2*>(grad_offsets)[wi] =
             make_float2(wgt * gw, wgt * gh);
@@ -288,7 +281,8 @@ __global__ void __launch_bounds__(kFusedBwdThreads) da_sca_bwd_kernel(
 #pragma unroll
     for (int z = 0; z < Z; ++z) {
       rxy[z] = __ldg(reinterpret_cast<const float2*>(ref_cam) + rbase + z);
-      bin[z] = depth_bin(__ldg(ref_depth + rbase + z), P);
+      bin[z] = depth_bin(__ldg(ref_depth + rbase + z), P.d_min, P.d_step,
+                         P.DC);
       dw[z] = sample_scalar(dp + bin[z], H0, W0, P.DC, pix(rxy[z].y, H0),
                             pix(rxy[z].x, W0));
       gdw[z] = 0.f;
@@ -318,14 +312,13 @@ __global__ void __launch_bounds__(kFusedBwdThreads) da_sca_bwd_kernel(
         const float a = w * dwz;
         const float h_im = pix(ly, H), w_im = pix(lx, W);
         float S, gh, gw;
-        sample_bwd<CH>(value + voff,
-                       !kDet && grad_value ? grad_value + voff : nullptr, H,
-                       W, E, h_im, w_im, a, G, S, gh, gw);
-        if (kDet && det.key && det_in_image(h_im, w_im, H, W)) {
-          const int64_t r = item * LP + (int64_t)l * P.points + p;
-          det.key[r] = det_value_key(h_im, w_im, W, pcell, P.heads, m);
-          det.rec[r] = make_float3(h_im, w_im, a);
-        }
+        sample_bwd<CH>(
+            value + voff, !kDet && grad_value ? grad_value + voff : nullptr,
+            H, W, E, h_im, w_im, a, G, S, gh, gw);
+        if (kDet && det.key && in_image(h_im, w_im, H, W))
+          det.value_record(item * LP + (int64_t)l * P.points + p,
+                           pcell + Bilinear(h_im, w_im).padded_cell(W),
+                           P.heads, m, h_im, w_im, a);
 #pragma unroll
         for (int z = 0; z < Z; ++z)
           if (zp == z) gdw[z] += w * S;
@@ -361,9 +354,9 @@ __global__ void __launch_bounds__(kFusedBwdThreads) da_sca_bwd_kernel(
 #pragma unroll
         for (int z = 0; z < Z; ++z) {
           const float h_im = pix(rxy[z].y, H0), w_im = pix(rxy[z].x, W0);
-          if (det_in_image(h_im, w_im, H0, W0)) {
+          if (in_image(h_im, w_im, H0, W0)) {
             det.dkey[slot + z] = (uint32_t)(
-                (n * cells + det_cell(h_im, w_im, W0)) * P.DC + bin[z]);
+                (n * cells + Bilinear(h_im, w_im).padded_cell(W0)) * P.DC + bin[z]);
             det.drec[slot + z] = make_float3(h_im, w_im, gdw[z]);
           }
         }
@@ -390,13 +383,14 @@ static int launch_msda_fused_bwd(
     cudaStream_t st) {
   const unsigned grid = (unsigned)ceil_div64(n_items, kFusedBwdThreads);
   count_launch();
-#define FBBEV_LAUNCH(CHV)                                                    \
-  msda_fused_bwd_kernel<CHV, kDet><<<grid, kFusedBwdThreads, 0, st>>>(       \
-      value, spatial_shapes, level_start, ref, offsets, logits, grad_out,    \
-      n_items, n_value, heads, levels, nq, points, grad_value, grad_offsets, \
-      grad_logits, det)
-  FBBEV_CH_DISPATCH(ch, FBBEV_LAUNCH)
-#undef FBBEV_LAUNCH
+  if (!dispatch(HeadWidths(), ch, [&](auto CH) {
+        msda_fused_bwd_kernel<CH.value, kDet>
+            <<<grid, kFusedBwdThreads, 0, st>>>(
+                value, spatial_shapes, level_start, ref, offsets, logits,
+                grad_out, n_items, n_value, heads, levels, nq, points,
+                grad_value, grad_offsets, grad_logits, det);
+      }))
+    return FBBEV_ERR_UNSUPPORTED;
   return launch_status();
 }
 
@@ -411,22 +405,17 @@ static int launch_da_sca_bwd(
     const DetSink& det, cudaStream_t st) {
   const unsigned grid = (unsigned)ceil_div64(n_items, kFusedBwdThreads);
   count_launch();
-#define FBBEV_LAUNCH_Z(CHV, ZV)                                              \
-  da_sca_bwd_kernel<CHV, ZV, kDet><<<grid, kFusedBwdThreads, 0, st>>>(       \
-      value, depth_prob, ref_cam, ref_depth, mask, offsets, logits,          \
-      spatial_shapes, level_start, P, grad_out, grad_value, grad_depth_prob, \
-      grad_offsets, grad_logits, det)
-#define FBBEV_LAUNCH(CHV)                                                    \
-  switch (Z) {                                                               \
-    case 1: FBBEV_LAUNCH_Z(CHV, 1); break;                                   \
-    case 2: FBBEV_LAUNCH_Z(CHV, 2); break;                                   \
-    case 4: FBBEV_LAUNCH_Z(CHV, 4); break;                                   \
-    case 8: FBBEV_LAUNCH_Z(CHV, 8); break;                                   \
-    default: return FBBEV_ERR_UNSUPPORTED;                                   \
-  }
-  FBBEV_CH_DISPATCH(ch, FBBEV_LAUNCH)
-#undef FBBEV_LAUNCH
-#undef FBBEV_LAUNCH_Z
+  bool launched = false;
+  dispatch(HeadWidths(), ch, [&](auto CH) {
+    launched = dispatch(ZAnchors(), Z, [&](auto ZV) {
+      da_sca_bwd_kernel<CH.value, ZV.value, kDet>
+          <<<grid, kFusedBwdThreads, 0, st>>>(
+              value, depth_prob, ref_cam, ref_depth, mask, offsets, logits,
+              spatial_shapes, level_start, P, grad_out, grad_value,
+              grad_depth_prob, grad_offsets, grad_logits, det);
+    });
+  });
+  if (!launched) return FBBEV_ERR_UNSUPPORTED;
   return launch_status();
 }
 
@@ -504,11 +493,8 @@ FBBEV_API int fbbev_da_sca_bwd(
       !vec_aligned(value, ch) || !vec_aligned(grad_out, ch) ||
       !vec_aligned(grad_value, ch))
     return FBBEV_ERR_INVALID_ARGUMENT;
-  DaScaParams P;
-  P.d_min = dbound_host[0];
-  P.d_step = dbound_host[2];
-  P.bs = bs; P.n_cams = n_cams; P.nq = nq; P.n_value = n_value;
-  P.heads = heads; P.levels = levels; P.points = points; P.DC = DC;
+  const DaScaParams P = da_sca_params(dbound_host, bs, n_cams, nq, n_value,
+                                      heads, levels, points, DC);
   return launch_da_sca_bwd<false>(
       value, depth_prob, ref_cam, ref_depth, mask, offsets, logits,
       spatial_shapes, level_start, P, ch, Z, n_items, grad_out, grad_value,

@@ -23,8 +23,6 @@
 // streamed operands only -- which the two fused entry points shrink further by
 // never materialising sampling_locations / normalised weights / the one-hot
 // depth tensor.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "da_sca_smem.h"
 #include "msda_common.cuh"
@@ -65,17 +63,10 @@ __device__ __forceinline__ void sample_accum(const float* __restrict__ val,
                                              int H, int W, int E, float h_im,
                                              float w_im, float wgt,
                                              float (&acc)[CH]) {
-  if (!(h_im > -1.f && w_im > -1.f && h_im < (float)H && w_im < (float)W))
-    return;
+  if (!in_image(h_im, w_im, H, W)) return;
   constexpr int VW = VecWidth<CH>::value;
-  const int h_low = (int)floorf(h_im), w_low = (int)floorf(w_im);
-  const int h_high = h_low + 1, w_high = w_low + 1;
-  const float lh = h_im - (float)h_low, lw = w_im - (float)w_low;
-  const float hh = 1.f - lh, hw = 1.f - lw;
-  const float w1 = hh * hw, w2 = hh * lw, w3 = lh * hw, w4 = lh * lw;
-  const bool t = h_low >= 0, btm = h_high <= H - 1;
-  const bool l = w_low >= 0, r = w_high <= W - 1;
-  const float* p1 = val + ((int64_t)h_low * W + w_low) * E;
+  const Bilinear bl(h_im, w_im);
+  const float* p1 = val + bl.offset(W, E);
   const float* p2 = p1 + E;
   const float* p3 = p1 + (int64_t)W * E;
   const float* p4 = p3 + E;
@@ -84,13 +75,14 @@ __device__ __forceinline__ void sample_accum(const float* __restrict__ val,
     float v1[10], v2[10], v3[10], v4[10];
 #pragma unroll
     for (int k = 0; k < 10; ++k) v1[k] = v2[k] = v3[k] = v4[k] = 0.f;
-    if (t && l) load10(p1, v1);
-    if (t && r) load10(p2, v2);
-    if (btm && l) load10(p3, v3);
-    if (btm && r) load10(p4, v4);
+    if (bl.ok1(H, W)) load10(p1, v1);
+    if (bl.ok2(H, W)) load10(p2, v2);
+    if (bl.ok3(H, W)) load10(p3, v3);
+    if (bl.ok4(H, W)) load10(p4, v4);
 #pragma unroll
     for (int k = 0; k < 10; ++k) {
-      const float s = w1 * v1[k] + w2 * v2[k] + w3 * v3[k] + w4 * v4[k];
+      const float s =
+          bl.w1 * v1[k] + bl.w2 * v2[k] + bl.w3 * v3[k] + bl.w4 * v4[k];
       acc[k] += s * wgt;
     }
     return;
@@ -100,13 +92,14 @@ __device__ __forceinline__ void sample_accum(const float* __restrict__ val,
     float v1[VW], v2[VW], v3[VW], v4[VW];
 #pragma unroll
     for (int k = 0; k < VW; ++k) v1[k] = v2[k] = v3[k] = v4[k] = 0.f;
-    if (t && l) load_vec<VW>(p1 + c, v1);
-    if (t && r) load_vec<VW>(p2 + c, v2);
-    if (btm && l) load_vec<VW>(p3 + c, v3);
-    if (btm && r) load_vec<VW>(p4 + c, v4);
+    if (bl.ok1(H, W)) load_vec<VW>(p1 + c, v1);
+    if (bl.ok2(H, W)) load_vec<VW>(p2 + c, v2);
+    if (bl.ok3(H, W)) load_vec<VW>(p3 + c, v3);
+    if (bl.ok4(H, W)) load_vec<VW>(p4 + c, v4);
 #pragma unroll
     for (int k = 0; k < VW; ++k) {
-      const float s = w1 * v1[k] + w2 * v2[k] + w3 * v3[k] + w4 * v4[k];
+      const float s =
+          bl.w1 * v1[k] + bl.w2 * v2[k] + bl.w3 * v3[k] + bl.w4 * v4[k];
       acc[c + k] += s * wgt;
     }
   }
@@ -297,7 +290,8 @@ __global__ void __launch_bounds__(kMsdaThreads) da_sca_fwd_kernel(
 #pragma unroll
     for (int z = 0; z < Z; ++z) {
       rxy[z] = __ldg(reinterpret_cast<const float2*>(ref_cam) + rbase + z);
-      const int bin = depth_bin(__ldg(ref_depth + rbase + z), P);
+      const int bin =
+          depth_bin(__ldg(ref_depth + rbase + z), P.d_min, P.d_step, P.DC);
       dw[z] = sample_scalar(dp + bin, H0, W0, P.DC, pix(rxy[z].y, H0),
                             pix(rxy[z].x, W0));
     }
@@ -379,21 +373,17 @@ FBBEV_API int fbbev_msda_fwd(const float* value, const int64_t* spatial_shapes,
   const unsigned grid = (unsigned)ceil_div64(n_items, kMsdaThreads);
   cudaStream_t st = as_stream(stream);
   count_launch();
-  if (!(ch == 4 || ch == 8 || ch == 10 || ch == 16 || ch == 20 || ch == 32 ||
-        ch == 64)) {
+  if (!dispatch(HeadWidths(), ch, [&](auto CH) {
+        msda_fwd_kernel<CH.value><<<grid, kMsdaThreads, 0, st>>>(
+            value, spatial_shapes, level_start, loc, attw, n_items, n_value,
+            heads, levels, nq, points, out);
+      })) {
     const int64_t n_out = n_items * ch;
     msda_fwd_generic_kernel<<<(unsigned)ceil_div64(n_out, kMsdaThreads),
                               kMsdaThreads, 0, st>>>(
         value, spatial_shapes, level_start, loc, attw, n_out, n_value, heads,
         ch, levels, nq, points, out);
-    return launch_status();
   }
-#define FBBEV_LAUNCH(CHV)                                                    \
-  msda_fwd_kernel<CHV><<<grid, kMsdaThreads, 0, st>>>(                       \
-      value, spatial_shapes, level_start, loc, attw, n_items, n_value, heads, \
-      levels, nq, points, out)
-  FBBEV_CH_DISPATCH(ch, FBBEV_LAUNCH)
-#undef FBBEV_LAUNCH
   return launch_status();
 }
 
@@ -416,37 +406,28 @@ FBBEV_API int fbbev_msda_fused_fwd(
   count_launch();
   if (patch_w > 0 && heads == 8 && levels == 1 && nq == n_value &&
       nq % patch_w == 0) {
-    // BEV self-attention: square query patches (see the kernel)
-    static int py = -1;  // FBBEV_MSDA_PATCH_Y: tuning aid (8 or 4 rows)
-    if (py < 0) {
-      const char* e = getenv("FBBEV_MSDA_PATCH_Y");
-      py = (e && atoi(e) == 4) ? 4 : 8;
-    }
+    // BEV self-attention: 8 x 8 query patches (see the kernel)
     constexpr int kPatch = 8;
     const int rows = nq / patch_w;
     const dim3 pgrid((unsigned)((patch_w + kPatch - 1) / kPatch),
-                     (unsigned)((rows + py - 1) / py), (unsigned)bs);
+                     (unsigned)((rows + kPatch - 1) / kPatch), (unsigned)bs);
     if (pgrid.y <= 65535 && pgrid.z <= 65535) {
-#define FBBEV_LAUNCH(CHV)                                                    \
-  if (py == 8)                                                               \
-    msda_fused_fwd_kernel<CHV, kPatch, 8><<<pgrid, kPatch * 64, 0, st>>>(    \
-        value, spatial_shapes, level_start, ref, offsets, logits, n_items,   \
-        n_value, heads, levels, nq, points, patch_w, out);                   \
-  else                                                                       \
-    msda_fused_fwd_kernel<CHV, kPatch, 4><<<pgrid, kPatch * 32, 0, st>>>(    \
-        value, spatial_shapes, level_start, ref, offsets, logits, n_items,   \
-        n_value, heads, levels, nq, points, patch_w, out)
-      FBBEV_CH_DISPATCH(ch, FBBEV_LAUNCH)
-#undef FBBEV_LAUNCH
+      if (!dispatch(HeadWidths(), ch, [&](auto CH) {
+            msda_fused_fwd_kernel<CH.value, kPatch, kPatch>
+                <<<pgrid, kPatch * kPatch * 8, 0, st>>>(
+                    value, spatial_shapes, level_start, ref, offsets, logits,
+                    n_items, n_value, heads, levels, nq, points, patch_w, out);
+          }))
+        return FBBEV_ERR_UNSUPPORTED;
       return launch_status();
     }
   }
-#define FBBEV_LAUNCH(CHV)                                                    \
-  msda_fused_fwd_kernel<CHV, 0, 0><<<grid, kMsdaThreads, 0, st>>>(              \
-      value, spatial_shapes, level_start, ref, offsets, logits, n_items,     \
-      n_value, heads, levels, nq, points, 0, out)
-  FBBEV_CH_DISPATCH(ch, FBBEV_LAUNCH)
-#undef FBBEV_LAUNCH
+  if (!dispatch(HeadWidths(), ch, [&](auto CH) {
+        msda_fused_fwd_kernel<CH.value, 0, 0><<<grid, kMsdaThreads, 0, st>>>(
+            value, spatial_shapes, level_start, ref, offsets, logits, n_items,
+            n_value, heads, levels, nq, points, 0, out);
+      }))
+    return FBBEV_ERR_UNSUPPORTED;
   return launch_status();
 }
 
@@ -468,11 +449,8 @@ FBBEV_API int fbbev_da_sca_fwd(
   if (!value || !depth_prob || !ref_cam || !ref_depth || !mask || !offsets ||
       !logits || !spatial_shapes || !level_start || !out)
     return FBBEV_ERR_INVALID_ARGUMENT;
-  DaScaParams P;
-  P.d_min = dbound_host[0];
-  P.d_step = dbound_host[2];
-  P.bs = bs; P.n_cams = n_cams; P.nq = nq; P.n_value = n_value;
-  P.heads = heads; P.levels = levels; P.points = points; P.DC = DC;
+  const DaScaParams P = da_sca_params(dbound_host, bs, n_cams, nq, n_value,
+                                      heads, levels, points, DC);
   const unsigned grid = (unsigned)ceil_div64(n_items, kMsdaThreads);
   cudaStream_t st = as_stream(stream);
   // whole camera map in shared memory when it fits (da_sca_smem.cu)
@@ -488,20 +466,14 @@ FBBEV_API int fbbev_da_sca_fwd(
                                             : (kScaPrologue | kScaMain));
   if (prologue_done) return FBBEV_ERR_INVALID_ARGUMENT;  // no such stage here
   count_launch();
-#define FBBEV_LAUNCH_Z(CHV, ZV)                                              \
-  da_sca_fwd_kernel<CHV, ZV><<<grid, kMsdaThreads, 0, st>>>(                 \
-      value, depth_prob, ref_cam, ref_depth, mask, offsets, logits,          \
-      spatial_shapes, level_start, P, out)
-#define FBBEV_LAUNCH(CHV)                                                    \
-  switch (Z) {                                                               \
-    case 1: FBBEV_LAUNCH_Z(CHV, 1); break;                                   \
-    case 2: FBBEV_LAUNCH_Z(CHV, 2); break;                                   \
-    case 4: FBBEV_LAUNCH_Z(CHV, 4); break;                                   \
-    case 8: FBBEV_LAUNCH_Z(CHV, 8); break;                                   \
-    default: return FBBEV_ERR_UNSUPPORTED;                                   \
-  }
-  FBBEV_CH_DISPATCH(ch, FBBEV_LAUNCH)
-#undef FBBEV_LAUNCH
-#undef FBBEV_LAUNCH_Z
+  bool launched = false;
+  dispatch(HeadWidths(), ch, [&](auto CH) {
+    launched = dispatch(ZAnchors(), Z, [&](auto ZV) {
+      da_sca_fwd_kernel<CH.value, ZV.value><<<grid, kMsdaThreads, 0, st>>>(
+          value, depth_prob, ref_cam, ref_depth, mask, offsets, logits,
+          spatial_shapes, level_start, P, out);
+    });
+  });
+  if (!launched) return FBBEV_ERR_UNSUPPORTED;
   return launch_status();
 }

@@ -52,8 +52,21 @@ def deterministic():
     return torch.are_deterministic_algorithms_enabled()
 
 
-def _workspace(nbytes, dev):
-    return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+def _run_backward(name, det, dev, args, ws_args):
+    """Calls backward entry point ``name`` with ``args`` on ``dev``'s current
+    stream; in deterministic mode its ``name + '_det'`` twin instead, with a
+    workspace sized by ``name + '_det_workspace_bytes'(*ws_args)``."""
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        if det:
+            name += '_det'
+            nb = getattr(L, name + '_workspace_bytes')(*ws_args)
+            ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=dev)
+            rc = getattr(L, name)(*args, _lib.ptr(ws), nb,
+                                  _lib.stream_ptr(dev))
+        else:
+            rc = getattr(L, name)(*args, _lib.stream_ptr(dev))
+    _lib.check(rc, name)
 
 
 def ms_deform_attn_forward(value, spatial_shapes, level_start_index,
@@ -108,31 +121,19 @@ class MultiScaleDeformableAttnFunction_fp32(Function):
         # samples outside the map leave their loc / attw gradient untouched
         grad_loc = torch.zeros_like(loc)
         grad_attw = torch.zeros_like(attw)
+        # the atomic kernel adds into grad_value; the deterministic one
+        # writes it whole
+        grad_value = (torch.empty_like if ctx.det else torch.zeros_like)(value)
         go = grad_output.contiguous().float()
         bs, n_value, heads, ch = value.shape
         _, nq, _, levels, points, _ = loc.shape
-        L = _lib.lib()
-        args = (_lib.ptr(value), _lib.ptr(ss), _lib.ptr(ls), _lib.ptr(loc),
-                _lib.ptr(attw), _lib.ptr(go), bs, n_value, heads, ch, levels,
-                nq, points)
-        with torch.cuda.device(dev):
-            if ctx.det:
-                grad_value = torch.empty_like(value)
-                nb = L.fbbev_msda_bwd_det_workspace_bytes(
-                    nq, n_value, heads, levels, points)
-                ws = _workspace(nb, dev)
-                name = 'fbbev_msda_bwd_det'
-                rc = L.fbbev_msda_bwd_det(
-                    *args, _lib.ptr(grad_value), _lib.ptr(grad_loc),
-                    _lib.ptr(grad_attw), _lib.ptr(ws), nb,
-                    _lib.stream_ptr(dev))
-            else:
-                grad_value = torch.zeros_like(value)
-                name = 'fbbev_msda_bwd'
-                rc = L.fbbev_msda_bwd(
-                    *args, _lib.ptr(grad_value), _lib.ptr(grad_loc),
-                    _lib.ptr(grad_attw), _lib.stream_ptr(dev))
-        _lib.check(rc, name)
+        _run_backward(
+            'fbbev_msda_bwd', ctx.det, dev,
+            (_lib.ptr(value), _lib.ptr(ss), _lib.ptr(ls), _lib.ptr(loc),
+             _lib.ptr(attw), _lib.ptr(go), bs, n_value, heads, ch, levels, nq,
+             points, _lib.ptr(grad_value), _lib.ptr(grad_loc),
+             _lib.ptr(grad_attw)),
+            (nq, n_value, heads, levels, points))
         return grad_value, None, None, grad_loc, grad_attw, None
 
 
@@ -172,8 +173,9 @@ def ms_deform_attn_fused(value, spatial_shapes, level_start_index,
     return out
 
 
-# head widths / anchor counts the fused kernels are built for
-# (FBBEV_CH_DISPATCH in csrc/msda_common.cuh; the Z switch of msda_fwd.cu)
+# head widths / anchor counts the fused kernels are built for (HeadWidths /
+# ZAnchors in csrc/msda_common.cuh; tests/test_fused_backward_abi.py checks
+# that the two agree)
 FUSED_HEAD_WIDTHS = (4, 8, 10, 16, 20, 32, 64)
 FUSED_Z_ANCHORS = (1, 2, 4, 8)
 
@@ -229,23 +231,13 @@ class MsdaFusedFunction(Function):
         go = grad_out.contiguous().float()
         bs, n_value, heads, ch = value.shape
         _, nq, _, levels, points, _ = off.shape
-        L = _lib.lib()
-        args = (_lib.ptr(value), _lib.ptr(ss), _lib.ptr(ls), _lib.ptr(ref),
-                _lib.ptr(off), _lib.ptr(lg), _lib.ptr(go), bs, n_value, heads,
-                ch, levels, nq, points, _lib.ptr(gv), _lib.ptr(goff),
-                _lib.ptr(glg))
-        with torch.cuda.device(dev):
-            if ctx.det:
-                nb = L.fbbev_msda_fused_bwd_det_workspace_bytes(
-                    nq, n_value, heads, levels, points)
-                ws = _workspace(nb, dev)
-                name = 'fbbev_msda_fused_bwd_det'
-                rc = L.fbbev_msda_fused_bwd_det(*args, _lib.ptr(ws), nb,
-                                                _lib.stream_ptr(dev))
-            else:
-                name = 'fbbev_msda_fused_bwd'
-                rc = L.fbbev_msda_fused_bwd(*args, _lib.stream_ptr(dev))
-        _lib.check(rc, name)
+        _run_backward(
+            'fbbev_msda_fused_bwd', ctx.det, dev,
+            (_lib.ptr(value), _lib.ptr(ss), _lib.ptr(ls), _lib.ptr(ref),
+             _lib.ptr(off), _lib.ptr(lg), _lib.ptr(go), bs, n_value, heads,
+             ch, levels, nq, points, _lib.ptr(gv), _lib.ptr(goff),
+             _lib.ptr(glg)),
+            (nq, n_value, heads, levels, points))
         return gv, None, None, None, goff, glg, None
 
 
@@ -495,25 +487,15 @@ class DaScaFunction(Function):
         n_cams, bs, nq, Z, _ = ref.shape
         _, _, _, levels, points, _ = off.shape
         DC = depth_prob.shape[-1]
-        L = _lib.lib()
-        args = (_lib.ptr(value), _lib.ptr(depth_prob), _lib.ptr(ref),
-                _lib.ptr(rdep), _lib.ptr(mask), _lib.ptr(off), _lib.ptr(lg),
-                _lib.ptr(ss), _lib.ptr(ls), _lib.c_floats(ctx.dbound),
-                _lib.ptr(go), bs, n_cams, nq, n_value, heads, ch, levels,
-                points, Z, DC, _lib.ptr(gv), _lib.ptr(gdp), _lib.ptr(goff),
-                _lib.ptr(glg))
-        with torch.cuda.device(dev):
-            if ctx.det:
-                nb = L.fbbev_da_sca_bwd_det_workspace_bytes(
-                    n_cams, nq, n_value, heads, ch, levels, points, Z, DC)
-                ws = _workspace(nb, dev)
-                name = 'fbbev_da_sca_bwd_det'
-                rc = L.fbbev_da_sca_bwd_det(*args, _lib.ptr(ws), nb,
-                                            _lib.stream_ptr(dev))
-            else:
-                name = 'fbbev_da_sca_bwd'
-                rc = L.fbbev_da_sca_bwd(*args, _lib.stream_ptr(dev))
-        _lib.check(rc, name)
+        _run_backward(
+            'fbbev_da_sca_bwd', ctx.det, dev,
+            (_lib.ptr(value), _lib.ptr(depth_prob), _lib.ptr(ref),
+             _lib.ptr(rdep), _lib.ptr(mask), _lib.ptr(off), _lib.ptr(lg),
+             _lib.ptr(ss), _lib.ptr(ls), _lib.c_floats(ctx.dbound),
+             _lib.ptr(go), bs, n_cams, nq, n_value, heads, ch, levels, points,
+             Z, DC, _lib.ptr(gv), _lib.ptr(gdp), _lib.ptr(goff),
+             _lib.ptr(glg)),
+            (n_cams, nq, n_value, heads, ch, levels, points, Z, DC))
         return (gv, gdp, None, None, None, goff, glg, None, None, None, None)
 
 

@@ -25,3 +25,29 @@ def test_fused_backward_argument_validation_without_gpu():
     assert da(1, 8, 4, None) == -1      # no dbound
     assert da(0, 8, 4) == 0             # empty: no-op
     assert da(0, 7, 4) == -1            # checked before the empty test
+
+
+def test_python_lists_match_library_without_gpu():
+    """FUSED_HEAD_WIDTHS / FUSED_Z_ANCHORS (what fused_grad_supported()
+    accepts) are exactly the head widths and Z counts the library's fused
+    kernels are built for: the _det entry points report FBBEV_ERR_UNSUPPORTED
+    (-3) for any other before their empty-problem test."""
+    from fbbev_b200 import _lib
+    from fbbev_b200.ops.ms_deform_attn import (FUSED_HEAD_WIDTHS,
+                                               FUSED_Z_ANCHORS)
+    L = _lib.lib()
+    for ch in range(1, 129):
+        # fbbev_msda_fused_bwd_det: 7 inputs, bs n_value heads ch levels nq
+        # points, 3 gradients, workspace, bytes, stream
+        rc = L.fbbev_msda_fused_bwd_det(*([None] * 7), 0, 10, 8, ch, 1, 5, 4,
+                                        None, None, None, None, 0, None)
+        assert rc == (0 if ch in FUSED_HEAD_WIDTHS else -3), (ch, rc)
+    dbound = _lib.c_floats([2.0, 42.0, 0.5])
+    for Z in range(1, 17):
+        # fbbev_da_sca_bwd_det: 9 inputs, dbound, grad_out, bs n_cams nq
+        # n_value heads ch levels points Z DC, 4 gradients, workspace, bytes,
+        # stream
+        rc = L.fbbev_da_sca_bwd_det(*([None] * 9), dbound, None, 0, 6, 10, 10,
+                                    8, 10, 1, 2 * Z, Z, 80, *([None] * 5), 0,
+                                    None)
+        assert rc == (0 if Z in FUSED_Z_ANCHORS else -3), (Z, rc)
