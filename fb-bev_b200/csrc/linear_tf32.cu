@@ -15,9 +15,14 @@
 // product is formed as 3xTF32 (see wg_kblock_3xtf32, wgmma.cuh): three
 // wgmma.mma_async kind tf32 per k8 step into the same fp32 accumulator.
 //
-// Structure: a persistent grid (as many CTAs as are resident at once), each
-// CTA looping over 128-row tiles; two warpgroups (rows 0-63 / 64-127 of the
-// tile).  The CTA's work is a sequence of steps, one per (tile, 40-float
+// Two kernels, chosen by the shape: for 40 < K <= 80 (every K of the encoder
+// layer) linear_tf32_kernel_resident keeps the weights in shared memory and
+// forms the A operands in registers (described at the kernel); every other K
+// runs linear_tf32_kernel, which streams the weights per K-block.
+//
+// linear_tf32_kernel: a persistent grid (as many CTAs as are resident at
+// once), each CTA looping over 128-row tiles; two warpgroups (rows 0-63 /
+// 64-127 of the tile).  The CTA's work is a sequence of steps, one per (tile, 40-float
 // K-block), through two shared-memory stages.  In step g each warpgroup issues
 // the full-width wgmma's of stage g & 1 (the tile's first with scale-d = 0),
 // then, once step g - 1's MMAs have drained, the CTA refills the other stage
@@ -89,19 +94,25 @@ struct LinearParams {
   int64_t ldy2;
   int n_split;
   float eps;
+  // resident-weight kernel: ring stages per warpgroup and the stage layout
+  // (bytes: X rows at 0, x_add rows at xa_off, residual rows at res_off)
+  int stages;
+  uint32_t stage_bytes, xa_off, res_off;
 };
 
 // Epilogue of one tile on the accumulator registers: bias, ReLU, residual,
 // LayerNorm (the four lanes of a quad hold one row: two shuffles per
 // reduction), column-pair stores (optionally split over two outputs).  `rbase`
 // is the thread's first row, q = lane % 4.  `cv` holds bias / gamma / beta
-// ([3][NPAD], zero past N) in shared memory, and the residual loads of a row
-// are issued in batches from always-valid addresses: a load that sits in a
-// branch in front of its use costs a full memory round trip per column pair.
-template <int NPAD, bool LN>
+// ([3][NPAD], zero past N) in shared memory.  `res(h, col)` returns residual
+// columns col, col + 1 of row rbase + 8 h; it is called from always-valid
+// addresses and in batches: a load that sits in a branch in front of its use
+// costs a full memory round trip per column pair.
+template <int NPAD, bool LN, typename Res>
 __device__ __forceinline__ void linear_epilogue(const LinearParams& p,
                                                 const float (&acc)[NPAD / 2],
-                                                const float* cv, int rbase, int q) {
+                                                const float* cv, int rbase, int q,
+                                                Res res) {
   constexpr int kBatch = 8;  // residual column pairs in flight per thread
   const int N = p.N;
 #pragma unroll
@@ -125,12 +136,8 @@ __device__ __forceinline__ void linear_epilogue(const LinearParams& p,
       for (int J0 = 0; J0 < NPAD / 8; J0 += kBatch) {
         float2 r[kBatch];
 #pragma unroll
-        for (int b = 0; b < kBatch && J0 + b < NPAD / 8; ++b) {
-          const int col = 8 * (J0 + b) + 2 * q;
-          const float* src = row_ok && col < N ? p.residual + (size_t)row * p.ldr + col
-                                               : p.residual;
-          r[b] = __ldg(reinterpret_cast<const float2*>(src));
-        }
+        for (int b = 0; b < kBatch && J0 + b < NPAD / 8; ++b)
+          r[b] = res(h, 8 * (J0 + b) + 2 * q);
 #pragma unroll
         for (int b = 0; b < kBatch && J0 + b < NPAD / 8; ++b) {
           t[2 * (J0 + b)] += r[b].x;
@@ -287,8 +294,13 @@ __global__ void __launch_bounds__(kLinThreads, 1)
     if (kb == n_kb - 1) {
       wgmma_wait<0>();
       acc_fence(acc);
-      linear_epilogue<NPAD, LN>(p, acc, cv, tile * kTileM + wg * 64 + wq * 16 + (lane >> 2),
-                                lane & 3);
+      const int rbase = tile * kTileM + wg * 64 + wq * 16 + (lane >> 2);
+      linear_epilogue<NPAD, LN>(p, acc, cv, rbase, lane & 3, [&](int h, int col) {
+        const int row = rbase + 8 * h;
+        const float* src = row < p.M && col < p.N ? p.residual + (size_t)row * p.ldr + col
+                                                  : p.residual;
+        return __ldg(reinterpret_cast<const float2*>(src));
+      });
       kb = 0;
       tile += gridDim.x;
     } else {
@@ -300,11 +312,200 @@ __global__ void __launch_bounds__(kLinThreads, 1)
   wgmma_wait<0>();  // nothing is pending (the last step ends in an epilogue)
 }
 
+// --------------------- resident-weight kernel (40 < K <= 80) ---------------------
+// The packed weights (two K-blocks, hi + lo: 10 KB per 16 columns) are copied
+// into shared memory once per CTA.  Each warpgroup works on its own 64-row
+// tiles (the CTA's tiles alternate between the two), so one warpgroup's
+// epilogue overlaps the other's MMAs and nothing synchronises the CTA after
+// the set-up.  A tile's rows are staged raw (fp32) in a per-warpgroup ring of
+// p.stages stages; within a stage each warp owns the 16 rows its A fragments
+// and accumulator rows cover, and fetches them itself: one 1-D bulk copy per
+// row and operand (X, x_add, residual), completion on the warp's own
+// mbarrier.  A warp reads only its own rows, so a stage needs no "empty"
+// barrier: the warp refills it as soon as it has read it -- right after the A
+// fragments are in registers when there is no residual, after the epilogue
+// otherwise.  The A operand is formed in registers: x (+ x_add, one fp32 add
+// as torch), hi = tf32_hi, lo = x - hi, and the same three MMAs per k8 step
+// as wg_kblock_3xtf32, in the same order.  X rows have a pitch of 84 floats,
+// which makes the fragment loads free of bank conflicts; residual rows have
+// NPAD + 8 (conflict-free float2 loads).
+constexpr int kRTileM = 64;
+constexpr int kXPitch = 84;
+constexpr int kMaxResidentK = 2 * kKB;
+constexpr int kMaxStages = 4;
+constexpr int kSmemLimit = 227 * 1024;  // opt-in shared memory per CTA (sm_90)
+
+template <int NPAD>
+constexpr uint32_t resident_w_bytes() { return 2u * 2u * NPAD * kKB * 4u; }
+
+// The MMAs of one 64-row tile over its two K-blocks, A from the raw stage in
+// registers: v = x + x_add (one fp32 add), hi = tf32_hi(v), lo = v - hi,
+// columns >= K zero; per k8 step the three products of wg_kblock_3xtf32 in
+// its order.  A K-block's fragments are formed before its fence, so the next
+// block's shared-memory loads overlap the MMAs of this one.
+template <int NPAD>
+__device__ __forceinline__ void resident_mma(float (&acc)[NPAD / 2], const float* xs,
+                                             const float* xa, int xa_pitch, int rl, int q,
+                                             int K, uint32_t w_base) {
+  constexpr uint32_t w_part = NPAD * kKB * 4;
+  uint32_t a_hi[2 * kKSteps][4], a_lo[2 * kKSteps][4];
+#pragma unroll
+  for (int kb = 0; kb < 2; ++kb) {
+#pragma unroll
+    for (int k = kb * kKSteps; k < (kb + 1) * kKSteps; ++k)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int r = rl + 8 * (e & 1), c = 8 * k + q + 4 * (e >> 1);
+        float v = __fadd_rn(xs[r * kXPitch + c], xa[r * xa_pitch + c]);
+        v = c < K ? v : 0.f;
+        const float hi = tf32_hi(v);
+        a_hi[k][e] = __float_as_uint(hi);
+        a_lo[k][e] = __float_as_uint(v - hi);
+      }
+    wgmma_fence();
+#pragma unroll
+    for (int k = kb * kKSteps; k < (kb + 1) * kKSteps; ++k) {
+      const uint32_t b_hi = w_base + kb * 2u * w_part + 2u * (k - kb * kKSteps) * NPAD * 16u;
+      const uint64_t dbh = smem_desc(b_hi, NPAD * 16, 128);
+      const uint64_t dbl = smem_desc(b_hi + w_part, NPAD * 16, 128);
+      wgmma_tf32_rs<NPAD>(acc, a_hi[k], dbh, k > 0);
+      wgmma_tf32_rs<NPAD>(acc, a_lo[k], dbh, 1u);
+      wgmma_tf32_rs<NPAD>(acc, a_hi[k], dbl, 1u);
+    }
+  }
+}
+
+template <int NPAD, bool LN>
+__global__ void __launch_bounds__(kLinThreads, 1)
+    linear_tf32_kernel_resident(const LinearParams p) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  constexpr uint32_t w_part = NPAD * kKB * 4;  // bytes of one K-block's W_hi
+  constexpr int kResPitch = NPAD + 8;
+  const int tid = threadIdx.x;
+  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
+  const int S = p.stages;
+  const uint32_t ring_bytes = 2u * S * p.stage_bytes;
+  unsigned char* ring = smem + resident_w_bytes<NPAD>() + wg * S * p.stage_bytes;
+  // mbarriers: [0] weights, then [warpgroup][stage][warp]
+  const uint32_t bars = smem_u32(smem + resident_w_bytes<NPAD>() + ring_bytes);
+  const uint32_t warp_bar = bars + 8u * (1 + wg * S * 4 + wq);  // + 32 s for stage s
+  float* cv = reinterpret_cast<float*>(smem + resident_w_bytes<NPAD>() + ring_bytes +
+                                       8 * (1 + 8 * S));  // [3][NPAD]
+  float* neg_zero = cv + 3 * NPAD;                         // [kMaxResidentK]
+  if (tid == 0) {
+    for (int i = 0; i <= 8 * S; ++i) mbar_init(bars + 8u * i, 1);
+    fence_mbar_init();
+  }
+  for (int i = tid; i < 3 * NPAD; i += kLinThreads) {
+    const int c = i % NPAD;
+    const float* v = i < NPAD ? p.bias : (i < 2 * NPAD ? p.gamma : p.beta);
+    cv[i] = v && c < p.N ? __ldg(v + c) : 0.f;
+  }
+  if (tid < kMaxResidentK) neg_zero[tid] = -0.f;
+  __syncthreads();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(bars, resident_w_bytes<NPAD>());
+    bulk_g2s(smem_u32(smem), p.wp, resident_w_bytes<NPAD>(), bars);
+  }
+
+  // this warpgroup's tiles: blockIdx.x + j gridDim.x for j = wg, wg + 2, ...
+  // (the grid is never larger than the tile count)
+  const int n_tiles = (p.M + kRTileM - 1) / kRTileM;
+  const int n_cta = (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1;
+  const int n_it = (n_cta - wg + 1) / 2;
+  const int K = p.K;
+  const uint32_t x_bytes = 4u * K;
+  const uint32_t row_bytes = x_bytes * (p.x_add ? 2u : 1u) + (p.residual ? 4u * p.N : 0u);
+  // warp-collective: stage the warp's 16 rows of tile iteration i
+  auto fill = [&](int i) {
+    if (i >= n_it) return;
+    const int s = i % S;
+    const int row0 = ((int)blockIdx.x + (2 * i + wg) * (int)gridDim.x) * kRTileM + 16 * wq;
+    const int rows = min(16, p.M - row0);  // may be <= 0 in the last tile
+    const uint32_t bar = warp_bar + 32u * s;
+    __syncwarp();
+    fence_proxy_async();  // the warp's reads of this stage before the copies' writes
+    if (lane == 0) mbar_arrive_expect_tx(bar, rows > 0 ? rows * row_bytes : 0u);
+    __syncwarp();
+    if (lane < rows) {
+      const int r = row0 + lane, lr = 16 * wq + lane;
+      unsigned char* st = ring + s * p.stage_bytes;
+      bulk_g2s(smem_u32(st + lr * kXPitch * 4), p.x + (size_t)r * p.ldx, x_bytes, bar);
+      if (p.x_add)
+        bulk_g2s(smem_u32(st + p.xa_off + lr * kXPitch * 4), p.x_add + (size_t)r * p.ldxa,
+                 x_bytes, bar);
+      if (p.residual)
+        bulk_g2s(smem_u32(st + p.res_off + lr * kResPitch * 4),
+                 p.residual + (size_t)r * p.ldr, 4u * p.N, bar);
+    }
+  };
+  for (int i = 0; i < S; ++i) fill(i);
+  mbar_wait(bars, 0);
+
+  const int rl = 16 * wq + (lane >> 2);  // stage row of acc[.. + 0 / 1]
+  const int q = lane & 3;
+  const uint32_t w_base = smem_u32(smem);
+  float acc[NPAD / 2];  // written first by a scale-d = 0 MMA, never zeroed
+  for (int i = 0; i < n_it; ++i) {
+    const int s = i % S;
+    mbar_wait(warp_bar + 32u * s, (uint32_t)(i / S) & 1u);
+    const unsigned char* st = ring + s * p.stage_bytes;
+    const float* xs = reinterpret_cast<const float*>(st);
+    // no x_add: add the row of -0 (x + -0 == x for every x), so the loads
+    // that define the A registers sit in no branch (ptxas would serialise the
+    // MMAs, C7520)
+    const float* xa = p.x_add ? reinterpret_cast<const float*>(st + p.xa_off) : neg_zero;
+    const int xa_pitch = p.x_add ? kXPitch : 0;
+    resident_mma<NPAD>(acc, xs, xa, xa_pitch, rl, q, K, w_base);
+    wgmma_commit();
+    if (!p.residual) fill(i + S);  // the stage is in registers: refill it now
+    wgmma_wait<0>();
+    acc_fence(acc);
+    const float* rs = reinterpret_cast<const float*>(st + p.res_off);
+    const int tile = (int)blockIdx.x + (2 * i + wg) * (int)gridDim.x;
+    linear_epilogue<NPAD, LN>(p, acc, cv, tile * kRTileM + rl, q, [&](int h, int col) {
+      return *reinterpret_cast<const float2*>(rs + (rl + 8 * h) * kResPitch + col);
+    });
+    if (p.residual) fill(i + S);
+  }
+}
+
 static inline int pad16(int n) { return (n + 15) / 16 * 16; }
 static inline int n_kblocks(int k) { return (k + kKB - 1) / kKB; }
 
+// Ring stages per warpgroup of the resident-weight kernel for this call, or
+// 0 (the streamed kernel runs) when the weights are not exactly two K-blocks
+// (40 < K <= 80) or they and one stage per warpgroup do not fit.
+static int resident_layout(LinearParams& p, int npad) {
+  if (p.n_kb != 2) return 0;
+  const uint32_t x_rows = kRTileM * kXPitch * 4;
+  p.xa_off = x_rows;
+  p.res_off = p.x_add ? 2 * x_rows : x_rows;
+  p.stage_bytes = p.res_off + (p.residual ? kRTileM * (npad + 8) * 4 : 0);
+  const int fixed = 2 * 2 * npad * kKB * 4 + 8 * (1 + 8 * kMaxStages) +
+                    (3 * npad + kMaxResidentK) * 4;
+  const int s = (kSmemLimit - fixed) / (2 * (int)p.stage_bytes);
+  return s < kMaxStages ? s : kMaxStages;
+}
+
 template <int NPAD, bool LN>
-static int launch_linear_t(const LinearParams& p, int tiles, cudaStream_t st) {
+static int launch_linear_t(const LinearParams& p, cudaStream_t st) {
+  if (p.stages > 0) {
+    static int resident = 0;  // CTAs that fit on the device at once
+    auto kern = linear_tf32_kernel_resident<NPAD, LN>;
+    if (!resident) {
+      cudaError_t e = cudaFuncSetAttribute(
+          kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
+      if (e != cudaSuccess) return (int)e;
+      e = resident_ctas(kern, kLinThreads, kSmemLimit, &resident);
+      if (e != cudaSuccess) return (int)e;
+    }
+    const size_t smem = resident_w_bytes<NPAD>() + 2 * (size_t)p.stages * p.stage_bytes +
+                        8 * (1 + 8 * p.stages) + (3 * NPAD + kMaxResidentK) * 4;
+    const int tiles = (int)ceil_div64(p.M, kRTileM);
+    kern<<<tiles < resident ? tiles : resident, kLinThreads, smem, st>>>(p);
+    return launch_status();
+  }
   constexpr size_t smem =
       2 * (2 * (size_t)kAPart + 2 * (size_t)NPAD * kKB * 4) + 16 + 3 * NPAD * 4;
   static int resident = 0;  // CTAs that fit on the device at once
@@ -316,25 +517,26 @@ static int launch_linear_t(const LinearParams& p, int tiles, cudaStream_t st) {
     e = resident_ctas(kern, kLinThreads, smem, &resident);
     if (e != cudaSuccess) return (int)e;
   }
+  const int tiles = (int)ceil_div64(p.M, kTileM);
   kern<<<tiles < resident ? tiles : resident, kLinThreads, smem, st>>>(p);
   return launch_status();
 }
 
 template <bool LN>
-static int launch_linear(const LinearParams& p, int npad, int tiles, cudaStream_t st) {
+static int launch_linear(const LinearParams& p, int npad, cudaStream_t st) {
   switch (npad) {
-    case 16: return launch_linear_t<16, LN>(p, tiles, st);
-    case 32: return launch_linear_t<32, LN>(p, tiles, st);
-    case 48: return launch_linear_t<48, LN>(p, tiles, st);
-    case 64: return launch_linear_t<64, LN>(p, tiles, st);
-    case 80: return launch_linear_t<80, LN>(p, tiles, st);
-    case 96: return launch_linear_t<96, LN>(p, tiles, st);
-    case 112: return launch_linear_t<112, LN>(p, tiles, st);
-    case 128: return launch_linear_t<128, LN>(p, tiles, st);
-    case 144: return launch_linear_t<144, LN>(p, tiles, st);
-    case 160: return launch_linear_t<160, LN>(p, tiles, st);
-    case 176: return launch_linear_t<176, LN>(p, tiles, st);
-    case 192: return launch_linear_t<192, LN>(p, tiles, st);
+    case 16: return launch_linear_t<16, LN>(p, st);
+    case 32: return launch_linear_t<32, LN>(p, st);
+    case 48: return launch_linear_t<48, LN>(p, st);
+    case 64: return launch_linear_t<64, LN>(p, st);
+    case 80: return launch_linear_t<80, LN>(p, st);
+    case 96: return launch_linear_t<96, LN>(p, st);
+    case 112: return launch_linear_t<112, LN>(p, st);
+    case 128: return launch_linear_t<128, LN>(p, st);
+    case 144: return launch_linear_t<144, LN>(p, st);
+    case 160: return launch_linear_t<160, LN>(p, st);
+    case 176: return launch_linear_t<176, LN>(p, st);
+    case 192: return launch_linear_t<192, LN>(p, st);
     default: return FBBEV_ERR_UNSUPPORTED;
   }
 }
@@ -395,11 +597,10 @@ static int linear_run(const float* x, int64_t ldx, const float* x_add,
   p.ldx = ldx; p.ldr = ldr; p.ldy = ldy;
   const bool ln = ln_weight != nullptr;
   if (ln && n > kMaxLnN) return FBBEV_ERR_UNSUPPORTED;
-  const int tiles = (int)ceil_div64(m, kTileM);
+  p.stages = resident_layout(p, pad16(n));
   cudaStream_t st = as_stream(stream);
   count_launch();
-  return ln ? launch_linear<true>(p, pad16(n), tiles, st)
-            : launch_linear<false>(p, pad16(n), tiles, st);
+  return ln ? launch_linear<true>(p, pad16(n), st) : launch_linear<false>(p, pad16(n), st);
 }
 
 FBBEV_API int fbbev_linear_fwd(const float* x, int64_t ldx, const float* packed,
