@@ -16,16 +16,23 @@
 //      words, one FMA per point and channel in point order,
 //      bev_pool_cuda.cu:36-40) and runs of equal voxel rank are stitched
 //      across groups through shared memory.  Interval sums go to compact rows
-//      V[interval][C] (43 MB for the 200x200x16 grid; they stay in L2), the
-//      part of an interval that spills into later slices to carry rows
-//      X[slice][C].
+//      V[interval][C] (43 MB for the 200x200x16 grid), the part of an
+//      interval that spills into later slices to carry rows X[slice][C].
 //  K2 "dense write": a CTA owns T consecutive voxel ranks x all C channels.
 //      Empty tiles stream zeros at once; the others copy the rows of their
 //      contiguous intervals V[i0:i1] into shared memory with cp.async, add
 //      carry rows in slice order, and stream the tile out channel row by channel
 //      row with 128-bit evict-first stores.
-//  Every output element and every V / X row is written exactly once; no
-//  atomics; results are deterministic.
+//  The one-shot op (K1 + K2 in one call) splits the work differently: most
+//  intervals are short (81 % one point, 97 % at most 8 on the 200x200x16
+//  grid), so K2 folds every interval of at most kShortLen points itself, in
+//  K1's exact summation order (IntervalFold), and K1 folds only the longer
+//  ones.  The index chase a tile then does is a few rounds of loads for ~24
+//  points; K2 starts beside K1 (programmatic dependent launch) and only the
+//  tiles holding a long interval (3 %) wait for it.
+//  The staged op (sums, then write / Z-mean) keeps the full V.
+//  Every output element is written exactly once, every V / X row at most
+//  once; no atomics; results are deterministic and the same on both paths.
 //
 // Requires C % 4 == 0 and (Z*Y*X) % 4 == 0, 16-byte aligned out.
 #include <algorithm>
@@ -52,6 +59,15 @@ __device__ __forceinline__ void cp_async_commit_wait_all() {
   asm volatile("cp.async.commit_group;" ::: "memory");
   asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
+// Programmatic dependent launch (sm_90): the primary grid lets its dependent
+// start early; the dependent waits for the primary's completion and memory
+// where it needs them.  Both are no-ops without such a dependency.
+__device__ __forceinline__ void grid_launch_dependents() {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+}
+__device__ __forceinline__ void grid_dependency_wait() {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+}
 
 // ------------------------------- plan --------------------------------------
 // tile_first[t] = first interval of tile t (tile_first[n_tiles] = n);
@@ -64,6 +80,67 @@ __device__ __forceinline__ void cp_async_commit_wait_all() {
 //                 tile-owning kernel's tail);
 // meta = {n_intervals, n_kept_points, n_warps}.
 constexpr int kPtsPerWarp = 32;
+
+// One-shot op: an interval of at most kShortLen points is folded by the dense
+// write itself, straight from feat / depth (97 % of the intervals of the
+// 200x200x16 grid, 81 % of them a single point); only the longer ones go
+// through K1 and V.
+constexpr int kShortLen = 8;
+
+// K1's point-group width LG for C channels (LG * VPL float4 columns cover C)
+__host__ __device__ inline int sum_group_width(int c4) {
+  return c4 <= 32 ? 4 : c4 <= 64 ? 8 : c4 <= 128 ? 16 : 32;
+}
+
+__device__ __forceinline__ float4 fma4(float4 x, float d, float4 a) {
+  return make_float4(fmaf(x.x, d, a.x), fmaf(x.y, d, a.y), fmaf(x.z, d, a.z),
+                     fmaf(x.w, d, a.w));
+}
+__device__ __forceinline__ float4 add4(float4 a, float4 b) {
+  return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+}
+
+// The sum of one interval in exactly K1 + K2's order, so that the dense write
+// can fold a short interval itself and match the staged V path bit for bit:
+//  - each LG-point group of the global point grid (points [LG*j, LG*j + LG))
+//    is one fmaf chain from +0, in point order;
+//  - within a 32-point slice (points [32*w, 32*w + 32)) the group partials are
+//    added left to right, the first one taken as it is (no +0 added);
+//  - the slice sums are added left to right (V row, then the carry rows X in
+//    slice order).
+// A one-point interval is therefore the rounded product fmaf(x, d, +0).
+// Feed the points in order with add(), the first one with first = true.
+struct IntervalFold {
+  float4 total, slice, group;
+  bool have_total, have_slice;
+  int lg_mask;
+  __device__ explicit IntervalFold(int lg) : have_total(false),
+      have_slice(false), lg_mask(lg - 1) {
+    group = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  __device__ void close_group() {
+    slice = have_slice ? add4(slice, group) : group;
+    have_slice = true;
+    group = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  __device__ void close_slice() {
+    total = have_total ? add4(total, slice) : slice;
+    have_total = true;
+    have_slice = false;
+  }
+  __device__ void add(int point, bool first, float4 x, float d) {
+    if (!first && (point & lg_mask) == 0) {
+      close_group();
+      if ((point & (kPtsPerWarp - 1)) == 0) close_slice();
+    }
+    group = fma4(x, d, group);
+  }
+  __device__ float4 result() {
+    close_group();
+    close_slice();
+    return total;
+  }
+};
 
 __global__ void split_plan_kernel(
     const int* __restrict__ ranks_bev, const int* __restrict__ interval_starts,
@@ -149,6 +226,12 @@ __device__ __forceinline__ void pool_trace(int slot, int tag, unsigned dep) {
 // part of an interval that started in an earlier slice goes to the slice's
 // carry row X[w] and is added, in slice order, by K2.  Every row is written
 // exactly once; no atomics; deterministic.
+// `long_only` (the one-shot op): K2 folds the intervals of at most kShortLen
+// points itself (IntervalFold), so a slice without a point of a longer
+// interval exits after its index loads.  A slice with one is folded whole: the
+// rows of its short intervals are written too but never read.  (Skipping their
+// points costs a per-run predicate in the fold loop, whose registers slow every
+// slice: 66.9 against 53.4 us on the 1-camera grid, an H100 SXM at 400 W.)
 template <int LG, int VPL>
 __global__ void __launch_bounds__(kSumThreads, FBBEV_SUM_MINB)
     interval_sums_kernel(const float* __restrict__ depth,
@@ -158,7 +241,7 @@ __global__ void __launch_bounds__(kSumThreads, FBBEV_SUM_MINB)
                          const int* __restrict__ ranks_bev,
                          const int* __restrict__ interval_starts,
                          const int* __restrict__ warp_first,
-                         const int* __restrict__ meta, int c,
+                         const int* __restrict__ meta, int c, int long_only,
                          float* __restrict__ V, float* __restrict__ X) {
   constexpr int WPC = kSumThreads / kWarp;
   constexpr int GPW = kWarp / LG;  // groups per warp
@@ -169,6 +252,7 @@ __global__ void __launch_bounds__(kSumThreads, FBBEV_SUM_MINB)
   const int trace_slot = blockIdx.x == 0 ? 0 : (blockIdx.x == gridDim.x - 8 ? 1 : -1);
 #endif
   PTRACE(0, 0);
+  grid_launch_dependents();  // the one-shot op's K2 may start beside K1
   if (w >= meta[2]) return;
   PTRACE(1, meta[2]);
   const int n = meta[0];
@@ -182,6 +266,16 @@ __global__ void __launch_bounds__(kSumThreads, FBBEV_SUM_MINB)
     rfL = __ldg(ranks_feat + base + lane);
     dL = __ldg(depth + __ldg(ranks_depth + base + lane));
   }
+  // long_only: an interval longer than kShortLen overlaps the slice exactly
+  // when two points kShortLen apart, the first in [base - kShortLen, base + 32),
+  // share a voxel rank.  The ranks of those pairs come with the index words,
+  // so the test delays none of the loads that follow.
+  int rbM = -2, rbP = -3;  // the ranks kShortLen before / 32 after this point
+  if (long_only) {
+    const int qm = base - kShortLen + lane, qp = base + kWarp + lane;
+    if (lane < cnt && qm >= 0) rbM = __ldg(ranks_bev + qm);
+    if (lane < kShortLen && qp < meta[1]) rbP = __ldg(ranks_bev + qp);
+  }
   PTRACE(2, rbL ^ rfL ^ lb);
   PTRACE(3, __float_as_uint(dL));
   // does the slice begin inside an interval that started earlier?
@@ -190,6 +284,11 @@ __global__ void __launch_bounds__(kSumThreads, FBBEV_SUM_MINB)
   const unsigned starts =
       __ballot_sync(kFull, lane < cnt && (lane == 0 || rbL != prev));
   PTRACE(4, starts ^ carry);
+  if (long_only) {  // a slice without a point of a long interval is done
+    const int rb24 = __shfl_sync(kFull, rbL, (kWarp - kShortLen + lane) & 31);
+    if (!__ballot_sync(kFull, rbM == rbL || (lane < kShortLen && rbP == rb24)))
+      return;
+  }
 
   const int gl = lane % LG, g = lane / LG, p0 = g * LG;
   const int c4 = c >> 2;
@@ -295,17 +394,28 @@ __global__ void __launch_bounds__(kSumThreads, FBBEV_SUM_MINB)
 // ---------------------------- K2: dense write ------------------------------
 // smem: rows[T + 1][c + 4] (row T stays zero: the row of an empty voxel)
 //       | slot[T] (row of each voxel) | carry_lo[T], carry_n[T] (carry rows
-//       X[lo+1 .. lo+n] of each interval)
+//       X[lo+1 .. lo+n] of each interval) | with fold_short: row_st[T],
+//       row_ln[T] (first point and length of each interval) and
+//       pt_rf[T][kShortLen], pt_rd[T][kShortLen] (index words of the points of
+//       the short intervals)
+// `fold_short` (the one-shot op; K1 ran with long_only): an interval of at
+// most kShortLen points is folded here, straight from feat / depth, instead of
+// copied from V.  The tile's loads go in rounds -- its interval words, then
+// the short intervals' index words, then their depth values and 128-bit feat
+// rows, all of a round in flight together -- and the stores follow the last.
+// The one-shot op launches K2 as a programmatic dependent of K1, so it runs
+// beside K1: only a tile that holds a long interval waits for K1 (griddepcontrol
+// .wait) before it reads V / X -- 3 % of the 64-voxel tiles at configs[1].
 template <int T>
 __global__ void __launch_bounds__(2 * T, 1280 / (2 * T)) dense_write_kernel(
     const float* __restrict__ V, const float* __restrict__ X,
     const int* __restrict__ tile_first, const int* __restrict__ seg_rank,
     const int* __restrict__ interval_starts,
     const int* __restrict__ interval_lengths, int c, int zyx,
-    const float* __restrict__ add, int yx_n, float* __restrict__ out, int part) {
-  // `part`: 0 every tile; 1 only the EMPTY tiles (their zero / `add` stream
-  // needs nothing but the plan, so it can run beside the interval sums); 2 only
-  // the tiles that hold intervals.
+    const float* __restrict__ add, int yx_n, float* __restrict__ out,
+    int fold_short, const float* __restrict__ depth,
+    const float* __restrict__ feat, const int* __restrict__ ranks_depth,
+    const int* __restrict__ ranks_feat) {
   // `add` (may be null): a (B, C, Y*X) map added to every Z slice while the
   // tile streams out -- FBOCC's `bev_feat_refined[..., None] + bev_feat`
   // (fbocc.py:365-366) without a second pass over the volume
@@ -315,17 +425,22 @@ __global__ void __launch_bounds__(2 * T, 1280 / (2 * T)) dense_write_kernel(
   int* slot = reinterpret_cast<int*>(rows + (size_t)(T + 1) * pitch);  // [T]
   int* carry_lo = slot + T;
   int* carry_n = carry_lo + T;
+  int* row_st = carry_n + T;
+  int* row_ln = row_st + T;
+  int* pt_rf = row_ln + T;
+  int* pt_rd = pt_rf + T * kShortLen;
 
   constexpr int kWrThreads = 2 * T, kWrWarps = kWrThreads / kWarp;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.y;
   const int tile = b * gridDim.x + blockIdx.x;
+  // the op is complete only once K1 is: one CTA waits for it
+  if (fold_short && tile == 0 && tid == 0) grid_dependency_wait();
   const int v0 = blockIdx.x * T;
   const int nv = min(T, zyx - v0);
   const int i0 = __ldg(tile_first + tile);
   const int i1 = __ldg(tile_first + tile + 1);
   const int nrows = min(i1 - i0, T);
-  if ((part == 1 && nrows > 0) || (part == 2 && nrows <= 0)) return;
   const int c4 = c >> 2;
   constexpr int LPR = T / 4;        // lanes per channel row
   constexpr int RPW = kWarp / LPR;  // rows per warp instruction
@@ -351,31 +466,56 @@ __global__ void __launch_bounds__(2 * T, 1280 / (2 * T)) dense_write_kernel(
     return;
   }
   // rows of this tile's intervals: contiguous in V, copied asynchronously,
-  // one warp per row
-  {
-    const float4* src = reinterpret_cast<const float4*>(V) + (int64_t)i0 * c4;
+  // one warp per row (with fold_short: the long intervals' rows, below)
+  const float4* V4 = reinterpret_cast<const float4*>(V);
+  if (!fold_short)
     for (int r = warp; r < nrows; r += kWrWarps)
       for (int v = lane; v < c4; v += kWarp)
-        cp_async16(rows + (size_t)r * pitch + 4 * v, src + (size_t)r * c4 + v);
-  }
+        cp_async16(rows + (size_t)r * pitch + 4 * v, V4 + (int64_t)(i0 + r) * c4 + v);
   for (int q = tid; q < T; q += kWrThreads) slot[q] = T;
   for (int q = tid; q < pitch; q += kWrThreads) rows[(size_t)T * pitch + q] = 0.f;
   __syncthreads();
   const int64_t rank0 = (int64_t)b * zyx + v0;
-  int any_carry = 0;
+  int any_carry = 0, any_long = 0;
   for (int r = tid; r < nrows; r += kWrThreads) {
     const int64_t vl = (int64_t)__ldg(seg_rank + i0 + r) - rank0;
     if (vl >= 0 && vl < nv) slot[vl] = r;
     const int st = __ldg(interval_starts + i0 + r);
     const int ln = __ldg(interval_lengths + i0 + r);
+    const bool from_v = !fold_short || ln > kShortLen;
     const int lo = st / kPtsPerWarp;
-    const int nx = (st + ln - 1) / kPtsPerWarp - lo;  // carry rows to add
+    const int nx = from_v ? (st + ln - 1) / kPtsPerWarp - lo : 0;  // carry rows
     carry_lo[r] = lo;
     carry_n[r] = nx;
     any_carry |= nx > 0;
+    if (fold_short) {
+      row_st[r] = st;
+      row_ln[r] = ln;
+      any_long |= from_v;
+    }
+  }
+  if (fold_short && __syncthreads_or(any_long)) {
+    grid_dependency_wait();  // V / X are K1's
+    for (int r = warp; r < nrows; r += kWrWarps)
+      if (row_ln[r] > kShortLen)
+        for (int v = lane; v < c4; v += kWarp)
+          cp_async16(rows + (size_t)r * pitch + 4 * v, V4 + (int64_t)(i0 + r) * c4 + v);
+  }
+  if (fold_short) {
+    // index words of the short intervals' points, slot [row][k]
+#pragma unroll
+    for (int k = 0; k < kShortLen / 2; ++k) {
+      const int q = tid + k * kWrThreads, r = q / kShortLen;
+      if (r < nrows && q % kShortLen < row_ln[r] && row_ln[r] <= kShortLen) {
+        const int p = row_st[r] + q % kShortLen;
+        pt_rf[q] = __ldg(ranks_feat + p);
+        pt_rd[q] = __ldg(ranks_depth + p);
+      }
+    }
   }
   cp_async_commit_wait_all();
-  if (__syncthreads_or(any_carry)) {
+  const bool carries = __syncthreads_or(any_carry);
+  if (carries) {
     // add the carry rows of intervals that span several K1 slices, in slice
     // order (deterministic); one warp per row, 8 loads in flight per lane
     const float4* X4 = reinterpret_cast<const float4*>(X);
@@ -402,8 +542,40 @@ __global__ void __launch_bounds__(2 * T, 1280 / (2 * T)) dense_write_kernel(
         *dst = a;
       }
     }
-    __syncthreads();
   }
+  if (fold_short) {
+    // the short intervals' rows, one (row, float4 column) per thread and pass;
+    // the depth and feat loads of two points in flight together (93 % of the
+    // intervals of the 200x200x16 grid have one or two points; four spill at
+    // the register budget of the launch bounds)
+    const float4* feat4 = reinterpret_cast<const float4*>(feat);
+    const int lg = sum_group_width(c4);
+    for (int j = tid; j < nrows * c4; j += kWrThreads) {
+      const int r = j / c4, v = j - r * c4;
+      const int ln = row_ln[r];
+      if (ln > kShortLen) continue;
+      const int st = row_st[r];
+      const int* rf = pt_rf + r * kShortLen;
+      const int* rd = pt_rd + r * kShortLen;
+      IntervalFold f(lg);
+      for (int k0 = 0; k0 < ln; k0 += 2) {
+        float4 x[2];
+        float d[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const bool in = k0 + k < ln;
+          d[k] = in ? __ldg(depth + rd[k0 + k]) : 0.f;
+          x[k] = in ? __ldg(feat4 + (int64_t)rf[k0 + k] * c4 + v)
+                    : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int k = 0; k < 2; ++k)
+          if (k0 + k < ln) f.add(st + k0 + k, k0 + k == 0, x[k], d[k]);
+      }
+      *reinterpret_cast<float4*>(rows + (size_t)r * pitch + 4 * v) = f.result();
+    }
+  }
+  if (carries || fold_short) __syncthreads();
 
   if (4 * g < nv) {
     // four consecutive voxels of one channel per lane; an empty voxel reads the
@@ -485,8 +657,9 @@ __global__ void __launch_bounds__(256) zmean_kernel(
   }
 }
 
-static inline size_t write_smem_bytes(int T, int c) {
-  return (size_t)(T + 1) * (c + 4) * 4 + (size_t)3 * T * 4;
+static inline size_t write_smem_bytes(int T, int c, bool fold_short = false) {
+  return (size_t)(T + 1) * (c + 4) * 4 + (size_t)3 * T * 4 +
+         (fold_short ? (size_t)(2 + 2 * kShortLen) * T * 4 : 0);
 }
 
 // FBBEV_POOL_TILE overrides the tile size (32 / 64 / 128 voxels) for tuning.
@@ -507,7 +680,7 @@ static int split_pick_tile(int c) {
 bool split_supported(int c, int64_t zyx) {
   return c % 4 == 0 && zyx % 4 == 0 && zyx < (1ll << 31) && c >= 4 &&
          c <= 1024 &&
-         write_smem_bytes(32, c) <= 200 * 1024;
+         write_smem_bytes(32, c, true) <= 200 * 1024;
 }
 
 static inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
@@ -590,63 +763,66 @@ int split_plan(const int* ranks_bev, const int* interval_starts,
   return launch_status();
 }
 
+// the point inputs the dense write folds short intervals from (fold_short)
+struct FoldInputs {
+  const float *depth, *feat;
+  const int *ranks_depth, *ranks_feat;
+};
+
+// K2; with `fold` (the one-shot op) as a programmatic dependent of the K1
+// launched just before it on `st` when `overlap`
 template <int T>
 static int launch_write(const SplitWs& w, const int* interval_starts,
                         const int* interval_lengths, int c, int64_t zyx,
                         int tiles_per_b, int batch, const float* add, int yx_n,
-                        float* out, cudaStream_t st, int part = 0) {
-  const size_t smem = write_smem_bytes(T, c);
+                        float* out, cudaStream_t st, const FoldInputs* fold,
+                        bool overlap) {
+  const size_t smem = write_smem_bytes(T, c, fold != nullptr);
   auto k = dense_write_kernel<T>;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(
         k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
   }
-  k<<<dim3((unsigned)tiles_per_b, (unsigned)batch), 2 * T, smem, st>>>(
-      w.V, w.X, w.tile_first, w.seg_rank, interval_starts, interval_lengths, c,
-      (int)zyx, add, yx_n, out, part);
+  const FoldInputs none = {nullptr, nullptr, nullptr, nullptr};
+  const FoldInputs& f = fold ? *fold : none;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)tiles_per_b, (unsigned)batch);
+  cfg.blockDim = dim3(2 * T);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = (fold && overlap) ? 1 : 0;
+  const cudaError_t e = cudaLaunchKernelEx(
+      &cfg, k, w.V, w.X, (const int*)w.tile_first, (const int*)w.seg_rank,
+      interval_starts, interval_lengths, c, (int)zyx, add, yx_n, out,
+      (int)(fold != nullptr), f.depth, f.feat, f.ranks_depth, f.ranks_feat);
+  if (e != cudaSuccess) return (int)e;
   return launch_status();
 }
 
 static int launch_write_any(int T, const SplitWs& w, const int* interval_starts,
                             const int* interval_lengths, int c, int64_t zyx,
                             int tiles_per_b, int batch, const float* add,
-                            int yx_n, float* out, cudaStream_t st, int part) {
+                            int yx_n, float* out, cudaStream_t st,
+                            const FoldInputs* fold, bool overlap) {
   switch (T) {
     case 128:
       return launch_write<128>(w, interval_starts, interval_lengths, c, zyx,
-                               tiles_per_b, batch, add, yx_n, out, st, part);
+                               tiles_per_b, batch, add, yx_n, out, st, fold,
+                               overlap);
     case 64:
       return launch_write<64>(w, interval_starts, interval_lengths, c, zyx,
-                              tiles_per_b, batch, add, yx_n, out, st, part);
+                              tiles_per_b, batch, add, yx_n, out, st, fold,
+                              overlap);
     default:
       return launch_write<32>(w, interval_starts, interval_lengths, c, zyx,
-                              tiles_per_b, batch, add, yx_n, out, st, part);
+                              tiles_per_b, batch, add, yx_n, out, st, fold,
+                              overlap);
   }
-}
-
-// Side stream for the zero stream of the empty tiles (one per host thread,
-// created on first use -- warm up once before capturing a CUDA graph).
-struct PoolSide {
-  cudaStream_t stream = nullptr;
-  cudaEvent_t fork = nullptr, join = nullptr;
-  int device = -1;
-};
-static PoolSide* pool_side() {
-  static thread_local PoolSide s;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (s.stream && s.device == dev) return &s;
-  if (s.stream) return nullptr;   // another device on this thread: no overlap
-  if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreateWithFlags(&s.fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&s.join, cudaEventDisableTiming) != cudaSuccess) {
-    s.stream = nullptr;
-    cudaGetLastError();
-    return nullptr;
-  }
-  s.device = dev;
-  return &s;
 }
 
 int split_launch(const float* depth, const float* feat, const int* ranks_depth,
@@ -666,23 +842,20 @@ int split_launch(const float* depth, const float* feat, const int* ranks_depth,
       split_layout(workspace, batch, zyx, n_intervals_max, n_points_max, c);
   const int T = split_pick_tile(c);
   const int tiles_per_b = (int)ceil_div64(zyx, T);
-  // One-shot op (sums + write): the empty tiles' zero stream -- 79 % of the
-  // 200x200x16 volume -- depends on the plan only, so it is launched on a side
-  // stream beside the interval sums (latency-bound, 18 us, few bytes) and the
-  // tiles that hold intervals follow the sums (FBBEV_POOL_OVERLAP=0: serial).
-  static const bool overlap_on = [] {
+  // One-shot op (sums + write): the dense write folds the intervals of at most
+  // kShortLen points itself and K1 only the longer ones, so only the tiles
+  // holding a long interval -- 302 of the 10,000 64-voxel tiles of the
+  // 200x200x16 grid at configs[1] -- need K1's rows.  K2 is launched as a
+  // programmatic dependent of K1: it starts beside K1 and only those tiles
+  // wait for it (FBBEV_POOL_OVERLAP=0: K2 after K1 in stream order).
+  // The staged op (sums, then write / Z-mean) keeps the full V.
+  const bool one_shot = do_sums && do_write && n_intervals_max > 0;
+  const FoldInputs fold_in = {depth, feat, ranks_depth, ranks_feat};
+  const FoldInputs* fold = one_shot ? &fold_in : nullptr;
+  static const bool overlap = [] {
     const char* e = getenv("FBBEV_POOL_OVERLAP");
     return !(e && e[0] == '0');
   }();
-  PoolSide* side = (do_sums && do_write && n_intervals_max > 0 && overlap_on)
-                       ? pool_side() : nullptr;
-  if (side) {
-    if (cudaEventRecord(side->fork, st) != cudaSuccess ||
-        cudaStreamWaitEvent(side->stream, side->fork, 0) != cudaSuccess) {
-      cudaGetLastError();
-      side = nullptr;
-    }
-  }
   if (do_sums && n_intervals_max > 0) {
     count_launch();
     const unsigned grid = (unsigned)w.n_sum_ctas;
@@ -690,36 +863,28 @@ int split_launch(const float* depth, const float* feat, const int* ranks_depth,
 #define FBBEV_SUM_CASE(LGV, VPLV)                                             \
   interval_sums_kernel<LGV, VPLV><<<grid, kSumThreads, 0, st>>>(              \
       depth, feat, ranks_depth, ranks_feat, ranks_bev, interval_starts,       \
-      w.warp_first, w.meta, c, w.V, w.X)
-    // group width LG and float4 columns per lane VPL with LG * VPL >= C / 4
-    if (c4 <= 4) FBBEV_SUM_CASE(4, 1);
-    else if (c4 <= 8) FBBEV_SUM_CASE(4, 2);
-    else if (c4 <= 16) FBBEV_SUM_CASE(4, 4);
-    else if (c4 <= 20) FBBEV_SUM_CASE(4, 5);
-    else if (c4 <= 32) FBBEV_SUM_CASE(4, 8);
-    else if (c4 <= 64) FBBEV_SUM_CASE(8, 8);
-    else if (c4 <= 128) FBBEV_SUM_CASE(16, 8);
+      w.warp_first, w.meta, c, fold != nullptr, w.V, w.X)
+    // group width LG = sum_group_width(C / 4) (the dense write's short-interval
+    // fold follows it) and float4 columns per lane VPL with LG * VPL >= C / 4
+    const int lg = sum_group_width(c4);
+    if (lg == 4) {
+      if (c4 <= 4) FBBEV_SUM_CASE(4, 1);
+      else if (c4 <= 8) FBBEV_SUM_CASE(4, 2);
+      else if (c4 <= 16) FBBEV_SUM_CASE(4, 4);
+      else if (c4 <= 20) FBBEV_SUM_CASE(4, 5);
+      else FBBEV_SUM_CASE(4, 8);
+    } else if (lg == 8) FBBEV_SUM_CASE(8, 8);
+    else if (lg == 16) FBBEV_SUM_CASE(16, 8);
     else FBBEV_SUM_CASE(32, 8);
 #undef FBBEV_SUM_CASE
     int rc = launch_status();
     if (rc) return rc;
   }
-  if (side) {   // after the sums: their CTAs take their SM slots first
-    count_launch();
-    int rc = launch_write_any(T, w, interval_starts, interval_lengths, c, zyx,
-                              tiles_per_b, batch, add, yx_n, out, side->stream, 1);
-    if (rc) return rc;
-  }
   if (!do_write) return FBBEV_OK;
   count_launch();
-  int rc = launch_write_any(T, w, interval_starts, interval_lengths, c, zyx,
-                            tiles_per_b, batch, add, yx_n, out, st, side ? 2 : 0);
-  if (side) {
-    if (cudaEventRecord(side->join, side->stream) != cudaSuccess ||
-        cudaStreamWaitEvent(st, side->join, 0) != cudaSuccess)
-      return (int)cudaGetLastError();
-  }
-  return rc;
+  return launch_write_any(T, w, interval_starts, interval_lengths, c, zyx,
+                          tiles_per_b, batch, add, yx_n, out, st, fold,
+                          overlap);
 }
 
 int split_zmean(const int* interval_starts, const int* interval_lengths,
