@@ -9,29 +9,56 @@
 // kernel, with the 40000 x 320 hidden activation (51 MB) written to and read
 // back from memory in between.  Here the hidden tile never leaves the SM:
 //
-//   X       the CTA's 128 rows of x, split hi / lo (3xTF32, see wgmma.cuh),
-//           stay in shared memory for the whole tile
-//   GEMM1   per 80-column hidden chunk: H[128 x 80] = X . W1_chunk^T, one
-//           wgmma accumulator per warpgroup (64 rows each)
-//   convert + b1, ReLU, hi / lo split of the accumulator registers into a
-//           shared-memory A tile (K-major core-matrix layout)
-//   GEMM2   Y[128 x E] += H_chunk . W2[:, chunk]^T, accumulator in registers
+//   X       a warpgroup's 64 rows of x, raw fp32 in shared memory (one 1-D bulk
+//           copy per row, 84-float pitch: conflict-free fragment loads), split
+//           hi / lo (3xTF32, see wgmma.cuh) into GEMM1's register A fragments
+//           one K-block at a time
+//   GEMM1   per 80-column hidden chunk: H[64 x 80] = X . W1_chunk^T, A from
+//           registers, accumulator in registers
+//   convert + b1, ReLU, hi / lo split of the accumulator registers into the
+//           warpgroup's rows of a shared-memory A tile (K-major core matrices)
+//   GEMM2   Y[64 x E] += H_chunk . W2[:, chunk]^T, accumulator in registers
 //           across all chunks
 //   finish  + b2 + residual, LayerNorm over the quad that holds each row,
 //           column-pair stores
 //
-// The grid is persistent (one CTA per SM), each CTA looping over 128-row
-// tiles.  The weights stream through a two-slot ring of 25.6 KB stages (one
-// 1-D bulk copy each, in the order the tensor cores consume them: the
-// K-blocks of W1 chunk c, then the two K-blocks of W2 that chunk c feeds; the
-// sequence runs on across the CTA's tiles).  Each stage is one full-width
-// wgmma per operand pair and k8 step; a slot is refilled as soon as the MMAs
-// of the stage before have drained (wgmma.wait_group 1), so the tensor cores
-// drain only at the hidden-chunk conversion.  The next tile's X rows are
-// loaded into registers during the last chunk and stored once its GEMM1 has
-// read the current tile.
-// Shared memory: X tile hi / lo (<= 80 KB) | hidden tile hi / lo (80 KB) |
-// weight ring (2 x 25.6 KB) | mbarriers | b1, b2, gamma, beta (2.2 KB).
+// The arithmetic is that of a plain chunk-by-chunk loop: per k8 step the three
+// products of wg_kblock_3xtf32 in its order, chunks into the GEMM2 accumulator
+// in hidden order (register A fragments give the same bits as the
+// shared-memory image of the same values).
+//
+// Work: rows are handed out in 64-row units, a contiguous run of
+// floor / ceil(units / grid) per CTA (at M = 40000: 625 units, 4 or 5 per
+// CTA, so the call lasts 2.5 steps of 128 rows rather than 3).  A CTA walks its
+// run two units per step, warpgroup w taking the step's unit w; when the run
+// is odd, warpgroup 1 sits out the last step.
+//
+// Weights stream through a four-slot ring of 25.6 KB stages (one 1-D bulk
+// copy each, in the order the MMAs are issued: per chunk the K-blocks of W1,
+// then the two of W2; the sequence runs on across the CTA's steps).  Both
+// warpgroups read every stage.  A slot has a "full" mbarrier (tx count) and an
+// arrival counter: each warp arrives once the MMAs reading the slot have
+// drained, and the warp whose arrival is the eighth refills the slot with the
+// stage four places on ("last one out refills": no producer warp, no warp
+// waits for a slot to empty).  Nothing synchronises the CTA after set-up; a
+// warpgroup's H rows need only a 128-thread named barrier, and each warp waits
+// for its own X rows on its own mbarrier.
+//
+// A warpgroup's chunk g, with GEMM2(g - 1) in flight on entry:
+//   issue GEMM1(g) (fragments formed per K-block, behind GEMM2(g - 1))
+//   wait for GEMM2(g - 1) only, release W2(g - 1): its slots refill while
+//     GEMM1(g) runs
+//   wait for GEMM1(g), release W1(g); at a tile edge, finish the previous tile
+//   convert g into H, named barrier, issue GEMM2(g)
+// Each refill has about one GEMM's MMAs to land in.  The finish and the
+// conversion run with the warpgroup's MMAs drained: an accumulator read while
+// any wgmma is in flight makes ptxas serialise every MMA (C7514), and a second
+// GEMM1 accumulator queued through the conversion does not fit the registers
+// beside the fragments at E > 40 (C7512).
+//
+// Shared memory: X rows (128 x 84 floats, 42 KB) | hidden tile hi / lo
+// (80 KB) | weight ring (4 x 25.6 KB) | mbarriers, counters | b1, b2, gamma,
+// beta (2.2 KB).
 //
 // Shapes: E <= 80, E % 4 == 0; hidden % 80 == 0, hidden <= 320.
 #include "common.cuh"
@@ -40,20 +67,25 @@
 namespace fbbev {
 namespace ffn {
 
-constexpr int kChunks = kKB / 4;        // 16-byte chunks of a row per K-block
 constexpr int kTileM = 128;
+constexpr int kUnitM = 64;              // rows per warpgroup and step
 constexpr int kAPart = kTileM * kKB * 4;            // bytes of A_hi (== A_lo)
 constexpr int kABlock = 2 * kAPart;                 // one K-block, hi + lo
 constexpr int kAChunkStride = (kTileM / 8) * 128;   // bytes between K chunks
 constexpr int kThreads = 256;           // two warpgroups
+constexpr int kWarps = kThreads / 32;
 constexpr int kHC = 80;                 // hidden columns per GEMM1 chunk
 constexpr int kMaxE = 80;
 constexpr int kMaxHidden = 320;
+constexpr int kXPitch = 84;             // floats per X row: conflict-free fragment loads
+constexpr int kSlots = 4;
 constexpr int kWStage = 2 * kHC * kKB * 4;          // >= 2 * pad16(E) * kKB * 4
-constexpr int kXBytes = 2 * kABlock;                // E <= 80: two K-blocks
+constexpr int kXBytes = kTileM * kXPitch * 4;
 constexpr int kHBytes = (kHC / kKB) * kABlock;
+constexpr int kBarBytes = 8 * (kSlots + kWarps) + 4 * kSlots + 16;
 constexpr int kCv = kMaxHidden + 3 * kMaxE;         // b1 | b2 | gamma | beta
-constexpr int kSmem = kXBytes + kHBytes + 2 * kWStage + 16 + kCv * 4;
+constexpr int kSmem = kXBytes + kHBytes + kSlots * kWStage + kBarBytes + kCv * 4;
+static_assert(kSmem <= 227 * 1024, "opt-in shared memory per CTA (sm_90)");
 
 struct Params {
   const float* x;         // [M][E]
@@ -65,7 +97,7 @@ struct Params {
   const float* gamma;     // [E] or null (no LayerNorm)
   const float* beta;
   float* y;               // [M][E]
-  int M, E, n_kb1, n_hc;
+  int M, E, n_hc;
   int64_t ldx, ldr, ldy;
   float eps;
 };
@@ -74,6 +106,20 @@ struct Params {
 __device__ __forceinline__ uint32_t a_off(int row, int col) {
   return (uint32_t)((col >> 2) * (kTileM / 8) + (row >> 3)) * 128u + (row & 7) * 16u +
          (col & 3) * 4u;
+}
+
+__device__ __forceinline__ void bar_sync_wg(int wg) {
+  asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+}
+// shared-memory counter add; acq_rel: the arriving warp's drained MMAs come
+// before the arrival, and the refill of the last arriver after all of them
+__device__ __forceinline__ uint32_t smem_add_acq_rel(uint32_t addr, uint32_t v) {
+  uint32_t old;
+  asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], %2;"
+               : "=r"(old)
+               : "r"(addr), "r"(v)
+               : "memory");
+  return old;
 }
 
 // finish of one tile on the GEMM2 accumulator: + b2 + residual, LayerNorm,
@@ -94,13 +140,11 @@ __device__ __forceinline__ void ffn_finish(const Params& p, const float (&acc2)[
     float t[NP2 / 4];
     float2 r[NP2 / 8];
     if (p.residual) {
+      // columns past E read the row's last pair (their sums are never used)
+      const float* res = p.residual + (row_ok ? (size_t)row * p.ldr : 0);
 #pragma unroll
-      for (int J = 0; J < NP2 / 8; ++J) {
-        const int col = 8 * J + 2 * q;
-        const float* src = row_ok && col < E ? p.residual + (size_t)row * p.ldr + col
-                                             : p.residual;
-        r[J] = __ldg(reinterpret_cast<const float2*>(src));
-      }
+      for (int J = 0; J < NP2 / 8; ++J)
+        r[J] = __ldg(reinterpret_cast<const float2*>(res + min(8 * J + 2 * q, E - 2)));
     }
 #pragma unroll
     for (int J = 0; J < NP2 / 8; ++J) {
@@ -156,23 +200,28 @@ __device__ __forceinline__ void ffn_finish(const Params& p, const float (&acc2)[
   }
 }
 
-template <int NP2>
+// NP2 = pad16(E); KB1 = 40-float K-blocks of E (GEMM1's stages per chunk)
+template <int NP2, int KB1>
 __global__ void __launch_bounds__(kThreads, 1) ffn_tf32_kernel(const Params p) {
   extern __shared__ __align__(128) unsigned char smem[];
-  unsigned char* xs = smem;
+  constexpr int per_c = KB1 + kHC / kKB;              // weight stages per chunk
+  const float* xrows = reinterpret_cast<const float*>(smem);
   unsigned char* hs = smem + kXBytes;
-  const uint32_t xs_a = smem_u32(xs), hs_a = smem_u32(hs);
+  const uint32_t hs_a = smem_u32(hs);
   const uint32_t ws_a = hs_a + kHBytes;
-  const uint32_t bar = ws_a + 2 * kWStage;
+  const uint32_t full = ws_a + kSlots * kWStage;      // [slot]
+  const uint32_t xbar = full + 8u * kSlots;           // [warp]
+  const uint32_t cnt = xbar + 8u * kWarps;            // [slot] arrival counters
   // b1 | b2 | gamma | beta, zero past hidden / E: read by every tile
-  float* cv = reinterpret_cast<float*>(hs + kHBytes + 2 * kWStage + 16);
+  float* cv = reinterpret_cast<float*>(hs + kHBytes + kSlots * kWStage + kBarBytes);
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
+  const int warp = tid >> 5;
   if (tid == 0) {
-    mbar_init(bar, 1);
-    mbar_init(bar + 8u, 1);
+    for (int i = 0; i < kSlots + kWarps; ++i) mbar_init(full + 8u * i, 1);
     fence_mbar_init();
   }
+  if (tid < kSlots) reinterpret_cast<uint32_t*>(smem + (cnt - smem_u32(smem)))[tid] = 0u;
   for (int i = tid; i < kCv; i += kThreads) {
     const int j = i < kMaxHidden ? i : (i - kMaxHidden) % kMaxE;
     const float* v = i < kMaxHidden ? p.b1
@@ -181,159 +230,213 @@ __global__ void __launch_bounds__(kThreads, 1) ffn_tf32_kernel(const Params p) {
     const int n = i < kMaxHidden ? p.n_hc * kHC : p.E;
     cv[i] = v && j < n ? __ldg(v + j) : 0.f;
   }
+  // the row copies write columns < E only: the columns past E stay zero
+  for (int i = tid; i < kXBytes / 16; i += kThreads)
+    reinterpret_cast<float4*>(smem)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   __syncthreads();
 
-  // tiles blockIdx.x, + gridDim.x, ... (the grid is never larger than the
-  // tile count); the weight stages of all of them form one sequence
-  const int n_tiles = (p.M + kTileM - 1) / kTileM;
-  const int per_c = p.n_kb1 + kHC / kKB;   // weight stages per hidden chunk
-  const int per_tile = p.n_hc * per_c;
-  const int total = ((n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1) * per_tile;
+  // this CTA's units [u0, u0 + n_units): steps of two, unit u0 + 2 s + wg
+  const int units = (p.M + kUnitM - 1) / kUnitM;
+  const int per = units / (int)gridDim.x, extra = units % (int)gridDim.x;
+  const int b = blockIdx.x;
+  const int u0 = b * per + min(b, extra);
+  const int n_units = per + (b < extra ? 1 : 0);
+  const int n_hc = p.n_hc;
+  const int n_chunks = (n_units + 1) / 2 * n_hc;          // the CTA's chunk sequence
+  const int my_chunks = (wg == 0 ? (n_units + 1) / 2 : n_units / 2) * n_hc;
+  // stage sequence, in the order the MMAs are issued: per chunk g the K-blocks
+  // of W1(g), then the two of W2(g).  Its length is read from shared memory
+  // by the refills, so that it takes no register in the chunk loop.
+  volatile int* total = reinterpret_cast<int*>(cv) - 4;
+  if (tid == 0) *total = n_chunks * per_c;
+  __syncthreads();
   auto issue_w = [&](int i) {
-    if (tid != 0 || i >= total) return;
-    const int t = i % per_tile;
-    const int c = t / per_c, j = t - c * per_c;
+    if (i >= *total) return;
+    const int g = i / per_c, t = i - g * per_c, c = g % n_hc;
     const float* src;
     uint32_t bytes;
-    if (j < p.n_kb1) {
-      src = p.w1p + (size_t)(c * p.n_kb1 + j) * (kWStage / 4);
+    if (t < KB1) {
+      src = p.w1p + (size_t)(c * KB1 + t) * (kWStage / 4);
       bytes = kWStage;
     } else {
-      const int kb = c * (kHC / kKB) + (j - p.n_kb1);
-      src = p.w2p + (size_t)kb * (2 * NP2 * kKB);
+      src = p.w2p + (size_t)(c * (kHC / kKB) + t - KB1) * (2 * NP2 * kKB);
       bytes = 2u * NP2 * kKB * 4u;
     }
-    const uint32_t s = i & 1;
-    mbar_arrive_expect_tx(bar + 8u * s, bytes);
-    bulk_g2s(ws_a + s * kWStage, src, bytes, bar + 8u * s);
+    const uint32_t s = i % kSlots;
+    mbar_arrive_expect_tx(full + 8u * s, bytes);
+    bulk_g2s(ws_a + s * kWStage, src, bytes, full + 8u * s);
   };
-  issue_w(0);
-  issue_w(1);
+  if (tid == 0)
+    for (int i = 0; i < kSlots; ++i) issue_w(i);
 
-  // X tile -> hi / lo images (columns >= E are zero): loaded into registers,
-  // then stored, so the next tile's loads overlap the current tile's tail
-  float4 xv[kXBytes / kABlock][5];
-  auto load_x = [&](int row0) {
-#pragma unroll
-    for (int kb = 0; kb < kXBytes / kABlock; ++kb)
-#pragma unroll
-      for (int i = 0; i < 5; ++i) {
-        const int idx = tid + kThreads * i;
-        const int r = idx / kChunks, ch = idx - r * kChunks;
-        const int g = row0 + r, col = kb * kKB + 4 * ch;
-        xv[kb][i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (kb < p.n_kb1 && g < p.M && col < p.E)
-          xv[kb][i] = __ldg(reinterpret_cast<const float4*>(p.x + (size_t)g * p.ldx + col));
-      }
-  };
-  auto store_x = [&]() {
-#pragma unroll
-    for (int kb = 0; kb < kXBytes / kABlock; ++kb) {
-      if (kb >= p.n_kb1) break;
-#pragma unroll
-      for (int i = 0; i < 5; ++i) {
-        const int idx = tid + kThreads * i;
-        const int r = idx / kChunks, ch = idx - r * kChunks;
-        const float4 v = xv[kb][i];
-        float4 hi;
-        hi.x = tf32_hi(v.x); hi.y = tf32_hi(v.y); hi.z = tf32_hi(v.z); hi.w = tf32_hi(v.w);
-        const float4 lo = make_float4(v.x - hi.x, v.y - hi.y, v.z - hi.z, v.w - hi.w);
-        unsigned char* a = xs + (size_t)kb * kABlock + a_off(r, 4 * ch);
-        *reinterpret_cast<float4*>(a) = hi;
-        *reinterpret_cast<float4*>(a + kAPart) = lo;
+  int it = 0;   // next stage to consume
+  int rel = 0;  // next stage to release
+  auto wait_stage = [&]() { mbar_wait(full + 8u * (it % kSlots), (it / kSlots) & 1u); };
+  // the warp's MMAs on stages [rel, rel + n) have drained: arrive; the eighth
+  // arrival refills the slot
+  auto release = [&](int n) {
+    for (int k = 0; k < n; ++k, ++rel) {
+      if (lane == 0) {
+        const uint32_t old = smem_add_acq_rel(cnt + 4u * (rel % kSlots), 1u);
+        if (old % kWarps == kWarps - 1) issue_w(rel + kSlots);
       }
     }
   };
-  load_x(blockIdx.x * kTileM);
-  store_x();
-  fence_proxy_async();
-  __syncthreads();
+  // stages this warpgroup does not read: still waited for (so the arrivals of
+  // one use of a slot never mix with the next) and released
+  auto skip = [&](int n) {
+    for (int k = 0; k < n; ++k) {
+      wait_stage();
+      ++it;
+      release(1);
+    }
+  };
+
+  // the warp's 16 X rows of step s, one bulk copy per row
+  const float* xw = xrows + (wg * kUnitM + 16 * wq) * kXPitch;
+  const uint32_t xb = xbar + 8u * warp;
+  auto fill_x = [&](int s) {
+    const int row0 = (u0 + 2 * s + wg) * kUnitM + 16 * wq;
+    const int rows = min(16, p.M - row0);  // may be <= 0 in the last unit
+    __syncwarp();
+    fence_proxy_async();  // the warp's reads of its rows before the copies' writes
+    if (lane == 0) mbar_arrive_expect_tx(xb, rows > 0 ? rows * 4u * p.E : 0u);
+    __syncwarp();
+    if (lane < rows)
+      bulk_g2s(smem_u32(xw + lane * kXPitch), p.x + (size_t)(row0 + lane) * p.ldx,
+               4u * p.E, xb);
+  };
+  // GEMM1's A fragments of one K-block of chunk gg's tile (hi / lo, columns
+  // >= E zero).  A tile's rows are waited for before its first K-block; after
+  // its last chunk's last K-block the warp's rows take the next tile's.
+  const int my_steps = my_chunks / n_hc;
+  auto frag = [&](uint32_t (&fh)[kKSteps][4], uint32_t (&fl)[kKSteps][4], int kb, int gg) {
+    const int s = gg / n_hc, c = gg - s * n_hc;
+    if (kb == 0 && c == 0) mbar_wait(xb, s & 1);
+#pragma unroll
+    for (int k = 0; k < kKSteps; ++k)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int r = (lane >> 2) + 8 * (e & 1), col = kb * kKB + 8 * k + q + 4 * (e >> 1);
+        const float v = xw[r * kXPitch + col];
+        const float hi = tf32_hi(v);
+        fh[k][e] = __float_as_uint(hi);
+        fl[k][e] = __float_as_uint(v - hi);
+      }
+    if (kb == KB1 - 1 && c == n_hc - 1 && s + 1 < my_steps) fill_x(s + 1);
+  };
+  // one K-block of GEMM1, one commit group
+  auto gemm1 = [&](float (&acc)[kHC / 2], const uint32_t (&fh)[kKSteps][4],
+                   const uint32_t (&fl)[kKSteps][4], int kb) {
+    wait_stage();
+    const uint32_t w_hi = ws_a + (it % kSlots) * kWStage;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kKSteps; ++k) {
+      const uint32_t b = w_hi + 2u * k * (kHC * 16);
+      const uint64_t dbh = smem_desc(b, kHC * 16, 128);
+      const uint64_t dbl = smem_desc(b + kHC * kKB * 4, kHC * 16, 128);
+      wgmma_tf32_rs<kHC>(acc, fh[k], dbh, kb > 0 || k > 0);
+      wgmma_tf32_rs<kHC>(acc, fl[k], dbh, 1u);
+      wgmma_tf32_rs<kHC>(acc, fh[k], dbl, 1u);
+    }
+    ++it;
+    wgmma_commit();
+  };
 
   const int rl = wg * 64 + wq * 16 + (lane >> 2);   // tile row of acc[.. + 0 / 1]
-  int it = 0;
-  // after issuing stage `it`'s wgmma's: once stage it - 1's have drained (both
-  // warpgroups), its slot takes stage it + 1 while stage it's MMAs run
-  auto next_stage = [&]() {
-    wgmma_commit();
-    wgmma_wait<1>();
-    __syncthreads();
-    if (it >= 1) issue_w(it + 1);
-    ++it;
-  };
-  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int row0 = tile * kTileM;
-    const bool more = tile + (int)gridDim.x < n_tiles;
-    float acc2[NP2 / 2];  // written first by a scale-d = 0 MMA, never zeroed
-    for (int c = 0; c < p.n_hc; ++c) {
-      float acc1[kHC / 2];
-      for (int j = 0; j < p.n_kb1; ++j) {
-        const uint32_t s = it & 1;
-        mbar_wait(bar + 8u * s, (it >> 1) & 1u);
-        const uint32_t a_hi = xs_a + j * kABlock + wg * 1024u;
-        const uint32_t w_hi = ws_a + s * kWStage;
-        wgmma_fence();
-        wg_kblock_3xtf32<kHC>(acc1, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
-                              w_hi + kHC * kKB * 4, kHC * 16, j > 0);
-        next_stage();
-      }
-      wgmma_wait<0>();
-      acc_fence(acc1);
-      // the last chunk's GEMM1 has read the X tile: the next tile's loads start
-      if (c == p.n_hc - 1 && more) load_x(row0 + (int)gridDim.x * kTileM);
-      // hidden chunk: + b1, ReLU, hi / lo split -> this warpgroup's rows of hs
+  unsigned char* const h_base = hs + a_off(rl, 2 * q);
+  float acc2[NP2 / 2];  // written first by a scale-d = 0 MMA, never zeroed
+  uint32_t f0h[kKSteps][4], f0l[kKSteps][4];  // K-block 0 of GEMM1
+  uint32_t f1h[kKSteps][4], f1l[kKSteps][4];  // K-block 1 (E > 40)
+  float acc1[kHC / 2];  // GEMM1 of the current chunk
+  // chunk g; GEMM2(g - 1) in flight on entry
+  auto chunk = [&](int g) {
+    const int c = g % n_hc;
+    frag(f0h, f0l, 0, g);
+    gemm1(acc1, f0h, f0l, 0);
+    if (KB1 == 2) {
+      frag(f1h, f1l, 1, g);
+      gemm1(acc1, f1h, f1l, 1);
+    }
+    if (g > 0) {
+      wgmma_wait<KB1>();  // GEMM2(g - 1) has drained, GEMM1(g) stays queued
+      release(kHC / kKB);
+    }
+    wgmma_wait<0>();
+    acc_fence(acc1);
+    release(KB1);
+    if (c == 0 && g > 0) {
+      // (after the full drain: ptxas serialises the MMAs when an accumulator
+      // is read while any wgmma is in flight, C7514)
+      acc_fence(acc2);
+      ffn_finish<NP2>(p, acc2, cv, (u0 + 2 * (g / n_hc - 1) + wg) * kUnitM + rl - wg * 64, q);
+    }
+    // hidden chunk: + b1, ReLU, hi / lo split -> this warpgroup's rows of hs
+    // (a_off(rl + 8 h, 8 J + 2 q + e) as the thread's base + a constant)
+    const float* b1c = cv + c * kHC + 2 * q;
 #pragma unroll
-      for (int J = 0; J < kHC / 8; ++J) {
+    for (int J = 0; J < kHC / 8; ++J) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int col = 8 * J + 2 * q + e;
-            float v = acc1[4 * J + 2 * h + e];
-            if (p.b1) v += cv[c * kHC + col];
-            v = fmaxf(v, 0.f);
-            const float hi = tf32_hi(v);
-            unsigned char* a = hs + (size_t)(col / kKB) * kABlock + a_off(rl + 8 * h, col % kKB);
-            *reinterpret_cast<float*>(a) = hi;
-            *reinterpret_cast<float*>(a + kAPart) = v - hi;
-          }
+        for (int e = 0; e < 2; ++e) {
+          float v = acc1[4 * J + 2 * h + e];
+          if (p.b1) v += b1c[8 * J + e];
+          v = fmaxf(v, 0.f);
+          const float hi = tf32_hi(v);
+          unsigned char* a = h_base + (J / kKSteps) * kABlock +
+                             (J % kKSteps) * 2 * kAChunkStride + h * 128 + e * 4;
+          *reinterpret_cast<float*>(a) = hi;
+          *reinterpret_cast<float*>(a + kAPart) = v - hi;
         }
       }
-      fence_proxy_async();
-      __syncthreads();
-      for (int j = 0; j < kHC / kKB; ++j) {
-        const uint32_t s = it & 1;
-        mbar_wait(bar + 8u * s, (it >> 1) & 1u);
-        const uint32_t a_hi = hs_a + j * kABlock + wg * 1024u;
-        const uint32_t w_hi = ws_a + s * kWStage;
-        wgmma_fence();
-        wg_kblock_3xtf32<NP2>(acc2, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
-                              w_hi + NP2 * kKB * 4, NP2 * 16, c > 0 || j > 0);
-        next_stage();
-      }
     }
-    // both warpgroups are past the last GEMM1 (the __syncthreads above)
-    if (more) store_x();
+    fence_proxy_async();
+    bar_sync_wg(wg);
+    // recomputed per chunk: hoisted out of the loop, the 20 descriptors would
+    // stay live across it
+    uint32_t h_a = hs_a + wg * 1024u;
+    asm volatile("" : "+r"(h_a));
+#pragma unroll
+    for (int j = 0; j < kHC / kKB; ++j) {
+      wait_stage();
+      const uint32_t a_hi = h_a + j * kABlock;
+      const uint32_t w_hi = ws_a + (it % kSlots) * kWStage;
+      wgmma_fence();
+      wg_kblock_3xtf32<NP2>(acc2, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
+                            w_hi + NP2 * kKB * 4, NP2 * 16, c > 0 || j > 0);
+      ++it;
+    }
+    wgmma_commit();
+  };
+
+  if (my_chunks > 0) {
+    fill_x(0);
+    for (int g = 0; g < my_chunks; ++g) chunk(g);
     wgmma_wait<0>();
     acc_fence(acc2);
-    ffn_finish<NP2>(p, acc2, cv, row0 + rl, q);
-    fence_proxy_async();
-    __syncthreads();
+    release(kHC / kKB);
+    ffn_finish<NP2>(p, acc2, cv, (u0 + 2 * (my_chunks / n_hc - 1) + wg) * kUnitM + rl - wg * 64,
+                    q);
   }
+  skip(*total - it);
 }
 
 static inline int pad16(int n) { return (n + 15) / 16 * 16; }
 
-template <int NP2>
-static int launch(const Params& p, int tiles, cudaStream_t st) {
+template <int NP2, int KB1>
+static int launch(const Params& p, cudaStream_t st) {
   static int resident = 0;  // CTAs that fit on the device at once
   if (!resident) {
     cudaError_t e = cudaFuncSetAttribute(
-        ffn_tf32_kernel<NP2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+        ffn_tf32_kernel<NP2, KB1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
     if (e != cudaSuccess) return (int)e;
-    e = resident_ctas(ffn_tf32_kernel<NP2>, kThreads, kSmem, &resident);
+    e = resident_ctas(ffn_tf32_kernel<NP2, KB1>, kThreads, kSmem, &resident);
     if (e != cudaSuccess) return (int)e;
   }
-  ffn_tf32_kernel<NP2><<<tiles < resident ? tiles : resident, kThreads, kSmem, st>>>(p);
+  const int steps = (int)ceil_div64(p.M, kTileM);  // two 64-row units per CTA at least
+  ffn_tf32_kernel<NP2, KB1><<<steps < resident ? steps : resident, kThreads, kSmem, st>>>(p);
   return launch_status();
 }
 
@@ -375,17 +478,16 @@ FBBEV_API int fbbev_ffn_fwd(const float* x, int64_t ldx, const float* w1_packed,
   p.x = x; p.w1p = w1_packed; p.b1 = b1; p.w2p = w2_packed; p.b2 = b2;
   p.residual = residual; p.gamma = ln_weight; p.beta = ln_bias; p.y = y;
   p.M = (int)m; p.E = embed;
-  p.n_kb1 = (embed + kKB - 1) / kKB;
   p.n_hc = hidden / ffn::kHC;
   p.ldx = ldx; p.ldr = ldr; p.ldy = ldy; p.eps = ln_eps;
-  const int tiles = (int)ceil_div64(m, ffn::kTileM);
   cudaStream_t st = as_stream(stream);
   count_launch();
+  const bool two_kb = embed > kKB;  // GEMM1 over two 40-float K-blocks
   switch (ffn::pad16(embed)) {
-    case 16: return ffn::launch<16>(p, tiles, st);
-    case 32: return ffn::launch<32>(p, tiles, st);
-    case 48: return ffn::launch<48>(p, tiles, st);
-    case 64: return ffn::launch<64>(p, tiles, st);
-    default: return ffn::launch<80>(p, tiles, st);
+    case 16: return ffn::launch<16, 1>(p, st);
+    case 32: return ffn::launch<32, 1>(p, st);
+    case 48: return two_kb ? ffn::launch<48, 2>(p, st) : ffn::launch<48, 1>(p, st);
+    case 64: return ffn::launch<64, 2>(p, st);
+    default: return ffn::launch<80, 2>(p, st);
   }
 }
