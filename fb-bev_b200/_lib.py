@@ -172,6 +172,11 @@ _SIGNATURES = {
     "fbbev_layernorm_bwd_workspace_bytes": (_sz, [_i64, _i32]),
     "fbbev_layernorm_bwd": (ctypes.c_int, [
         _p, _i64, _p, _p, _p, _i64, _i32, _p, _i64, _p, _p, _p, _sz, _p]),
+    "fbbev_depth_loss_workspace_bytes": (_sz, [_i32, _i32, _i32]),
+    "fbbev_depth_loss_fwd": (ctypes.c_int, [_p, _p] + [_i32] * 5 + [
+        ctypes.c_float] * 3 + [_p, _p, _p, _p, _sz, _p]),
+    "fbbev_depth_loss_bwd": (ctypes.c_int, [_p] * 4 + [_i32] * 4 + [
+        ctypes.c_float, _p, _p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
@@ -237,7 +242,8 @@ class KernelTimer:
              "fbbev_history_train_full_workspace_bytes",
              "fbbev_history_warp_bwd_workspace_bytes",
              "fbbev_history_restart_grad_workspace_bytes",
-             "fbbev_layernorm_bwd_workspace_bytes")
+             "fbbev_layernorm_bwd_workspace_bytes",
+             "fbbev_depth_loss_workspace_bytes")
 
     def __init__(self):
         self.records = []   # (name, args, start_event, end_event)

@@ -86,11 +86,27 @@ def make_cam_params(batch=1, n_cams=6, input_size=(256, 704),
                  (rots, trans, intr, post_rots, post_trans, bda))
 
 
+# torch's CPU softmax over a dim that is not the innermost one splits the
+# inner extent across the intra-op threads, and the vectorised exp rounds
+# differently from the scalar loop that finishes each chunk: the same seed gives
+# other last bits on a host with another thread count.  The depth maps are
+# evaluated with this fixed count, so a seed means the same tensor on every
+# (x86, AVX2 / AVX-512) host; it is the count the committed fixtures built from
+# these inputs (tests/golden/r_ref_cuda.npz) were recorded with.
+SOFTMAX_THREADS = 16
+
+
 def make_depth_feat(batch, n_cams, D, H, W, C, device="cpu", seed=0):
     """``depth = softmax(randn)`` over D (B,N,D,H,W) and ``feat = randn``
     (B,N,C,H,W) -- the outputs of CM_DepthNet (modules/depth_net.py:335-366)."""
     g = torch.Generator().manual_seed(seed)
-    depth = torch.randn(batch, n_cams, D, H, W, generator=g).softmax(dim=2)
+    logits = torch.randn(batch, n_cams, D, H, W, generator=g)
+    threads = torch.get_num_threads()
+    torch.set_num_threads(SOFTMAX_THREADS)
+    try:
+        depth = logits.softmax(dim=2)
+    finally:
+        torch.set_num_threads(threads)
     g.manual_seed(seed + 1)
     feat = torch.randn(batch, n_cams, C, H, W, generator=g)
     return depth.to(device), feat.to(device)

@@ -25,6 +25,7 @@ the step before the path.
 import torch
 import torch.nn as nn
 
+from ..ops import depth_loss as _depth_loss
 from ..ops.bev_pool_v2 import (voxel_pooling_prepare_from_cams,
                                voxel_pooling_prepare_v2)
 from ..ops.lift_tail import lift_tail
@@ -228,6 +229,24 @@ class LSSViewTransformerBEVDepth(LSSViewTransformer2):
         sensor2ego = torch.cat([rot, tran.reshape(B, N, 3, 1)],
                                dim=-1).reshape(B, N, -1)
         return torch.cat([mlp_input, sensor2ego], dim=-1)
+
+    # -- :1036-1065 --------------------------------------------------------
+    def get_downsampled_gt_depth(self, gt_depths):
+        """gt_depths (B, N, H, W) -> float one-hot (B*N*h*w, D)."""
+        return _depth_loss.downsampled_gt_depth(
+            gt_depths, self.downsample, self.grid_config['depth'], self.D)
+
+    # -- :1067-1081 --------------------------------------------------------
+    def get_depth_loss(self, depth_labels, depth_preds):
+        """depth_labels: gt depth (B, N, H, W); depth_preds (B*N, D, h, w).
+        Returns the weighted 0-d loss, computed without a host sync."""
+        if depth_preds.shape[1] != self.D:
+            raise ValueError(f'depth_preds has {depth_preds.shape[1]} bins, '
+                             f'the grid has {self.D}')
+        return _depth_loss.depth_loss(depth_labels, depth_preds,
+                                      self.downsample,
+                                      self.grid_config['depth'],
+                                      self.loss_depth_weight)
 
     def _depth_net_out(self, input):
         x, mlp_input = input[0], input[7]

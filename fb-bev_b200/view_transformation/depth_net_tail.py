@@ -25,12 +25,16 @@ kernels read:
   ``fbbev_lift_tail_fwd`` launch.
 
 ``LSSViewTransformerFunction3D.forward(..., context_layout='nhwc')`` takes the
-result as it is.  The body of the depth net (ResNet blocks, ASPP, DCN, the SE
-gates) is the step before and stays what it is (SURVEY.md section 2).
+result as it is.  ``get_depth_loss`` / ``get_downsampled_gt_depth``
+(depth_net.py:396-450), the depth supervision FB-OCC trains with, run on the
+``fbbev_depth_loss_*`` kernels (ops/depth_loss.py) without a host sync.  The
+body of the depth net (ResNet blocks, ASPP, DCN, the SE gates) is the step
+before and stays what it is (SURVEY.md section 2).
 """
 import torch
 import torch.nn as nn
 
+from ..ops import depth_loss as _depth_loss
 from ..ops import linear as _linear_ops
 from ..ops.lift_tail import lift_tail
 from ..registry import BaseModule
@@ -43,11 +47,28 @@ class CM_DepthNetTail(BaseModule):
 
     The parameter name (``context_conv.{weight,bias}``) is the reference's, so
     ``tail.load_state_dict(depth_net.state_dict(), strict=False)`` adopts a
-    trained CM_DepthNet's weights."""
+    trained CM_DepthNet's weights.
 
-    def __init__(self, mid_channels=512, context_channels=64):
+    ``downsample``, ``grid_config``, ``depth_channels``, ``loss_depth_weight``
+    and ``sid`` are the reference's depth-supervision keywords (plain
+    attributes, no state).  ``depth_channels=None`` takes D from the logits
+    (``get_depth_loss``) or from ``grid_config['depth']``
+    (``get_downsampled_gt_depth``); ``sid=True`` is not supported."""
+
+    def __init__(self, mid_channels=512, context_channels=64, downsample=16,
+                 grid_config=None, depth_channels=None, loss_depth_weight=3.0,
+                 sid=False):
         super().__init__()
+        if sid:
+            raise NotImplementedError(
+                'CM_DepthNetTail: sid=True (spacing-increasing depth bins) is '
+                'not supported')
         self.context_channels = context_channels
+        self.downsample = downsample
+        self.grid_config = grid_config
+        self.depth_channels = depth_channels
+        self.loss_depth_weight = loss_depth_weight
+        self.sid = sid
         self.context_conv = nn.Conv2d(mid_channels, context_channels,
                                       kernel_size=1, stride=1, padding=0)
 
@@ -73,6 +94,33 @@ class CM_DepthNetTail(BaseModule):
                                     self.context_conv(context_feat))
             feat = feat.view(B, N, H, W, C)
         return feat, depth.view(B, N, D, H, W)
+
+    def _depth_cfg(self):
+        if self.grid_config is None:
+            raise ValueError('CM_DepthNetTail: the depth loss needs grid_config')
+        return self.grid_config['depth']
+
+    # -- depth_net.py:396-434 ----------------------------------------------
+    def get_downsampled_gt_depth(self, gt_depths):
+        """gt_depths (B, N, H, W) -> float one-hot (B*N*h*w, D)."""
+        cfg = self._depth_cfg()
+        D = self.depth_channels
+        if D is None:
+            D = torch.arange(*cfg, dtype=torch.float).shape[0]
+        return _depth_loss.downsampled_gt_depth(gt_depths, self.downsample,
+                                                cfg, D)
+
+    # -- depth_net.py:436-450 ----------------------------------------------
+    def get_depth_loss(self, depth_labels, depth_preds):
+        """depth_labels: gt depth (B, N, H, W); depth_preds (B, N, D, h, w).
+        Returns ``dict(loss_depth=0-d tensor)``."""
+        D = depth_preds.shape[2]
+        if self.depth_channels is not None and D != self.depth_channels:
+            raise ValueError(f'depth_preds has {D} bins, depth_channels is '
+                             f'{self.depth_channels}')
+        return dict(loss_depth=_depth_loss.depth_loss(
+            depth_labels, depth_preds, self.downsample, self._depth_cfg(),
+            self.loss_depth_weight))
 
 
 def _softmax_only(depth_logits):

@@ -1154,6 +1154,56 @@ int fbbev_history_restart_grad_curr(
     int32_t W, float* grad_curr, void* workspace, size_t workspace_bytes,
     fbbev_stream_t stream);
 
+/* =====================================================================
+ * D -- depth supervision of the lift step (the training loss on `depth`)
+ * ===================================================================== */
+
+/*
+ * Replaces get_downsampled_gt_depth + get_depth_loss of CM_DepthNet
+ *   mmdet3d/models/fbbev/modules/depth_net.py:396-450
+ * and of LSSViewTransformerBEVDepth
+ *   mmdet3d/models/necks/view_transformer.py:1036-1081
+ * (sid = False) with no host synchronisation.
+ * gt (bn, H, W) fp32 dense; preds (bn, d, h, w) fp32 dense, h = H / ds,
+ * w = W / ds (CM's (B, N, D, h, w) is the same memory).
+ *   m     = min over the ds x ds patch of (g == 0 ? 1e5 : g), NaN propagating
+ *   t     = (m - c0) * (1 / c1)     fp32, as torch's CUDA division by a scalar
+ *   label = (0 <= t < d + 1) ? trunc(t) : 0             class in [0, d]
+ * with c0 = (float)(lo - step) (difference in double), c1 = (float)step of
+ * grid_config['depth'] = [lo, hi, step].  Pixels with label >= 1 are
+ * foreground, one-hot at bin label - 1.
+ *   loss = weight * (S / max(1, n_fg)),  S = sum over foreground pixels and
+ *   all d bins of torch's binary_cross_entropy element (logs clamped at -100)
+ * Outputs: labels (bn, h, w) int32 -- the only per-pixel state the backward
+ * needs; loss (0-d fp32) and n_fg (0-d int32) on the device.  The sum is
+ * deterministic (per-row partials in the workspace, added in a fixed order;
+ * no float atomics).
+ * preds == NULL computes labels only (loss, n_fg and the workspace unused,
+ * loss and n_fg must be NULL).
+ * workspace: fbbev_depth_loss_workspace_bytes(bn, H, ds) bytes, 16-byte
+ * aligned.  Errors: H or W not a multiple of ds, d <= 0, NULL or misaligned
+ * pointers.  bn == 0 is a no-op.  W <= 12288 (else FBBEV_ERR_UNSUPPORTED).
+ */
+size_t fbbev_depth_loss_workspace_bytes(int32_t bn, int32_t H, int32_t ds);
+int fbbev_depth_loss_fwd(const float* gt, const float* preds, int32_t bn,
+                         int32_t H, int32_t W, int32_t ds, int32_t d, float c0,
+                         float c1, float weight, int32_t* labels, float* loss,
+                         int32_t* n_fg, void* workspace,
+                         size_t workspace_bytes, fbbev_stream_t stream);
+/*
+ * d preds of fbbev_depth_loss_fwd's loss, dense (bn, d, h, w), 0 at
+ * background pixels; grad_loss: device fp32 scalar (the upstream gradient),
+ * n_fg as the forward wrote it.  In the reference's autograd order:
+ *   k = (grad_loss * weight) / max(1, n_fg)
+ *   grad_preds = k * (p - y) / max((1 - p) * p, 1e-12)
+ * each an IEEE fp32 operation.  bn == 0 is a no-op.
+ */
+int fbbev_depth_loss_bwd(const int32_t* labels, const float* preds,
+                         const int32_t* n_fg, const float* grad_loss,
+                         int32_t bn, int32_t h, int32_t w, int32_t d,
+                         float weight, float* grad_preds,
+                         fbbev_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
