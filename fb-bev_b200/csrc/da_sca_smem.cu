@@ -35,8 +35,6 @@
 // Used when the whole map fits (n_value * E * 4 <= ~220 KB) for the head layout
 // the bank analysis holds for (8 heads x 10 channels, 1 level, 8 points, 4
 // anchors); every other shape keeps the global-memory kernel.
-#include <stdlib.h>
-
 #include "bulk.cuh"
 #include "common.cuh"
 #include "da_sca_smem.h"
@@ -421,26 +419,18 @@ int da_sca_smem_launch(const float* value, const float* depth_prob,
     if (!(stages & kScaMain)) return launch_status();
   }
   count_launch();
-  // 512 or 640 threads per CTA (FBBEV_SCA_THREADS: tuning aid)
-  static int threads = 0;
-  if (threads == 0) {
-    const char* e = getenv("FBBEV_SCA_THREADS");
-    threads = (e && atoi(e) == 640) ? 640 : 512;
+  static bool smem_opt_in = false;
+  if (!smem_opt_in) {
     cudaFuncSetAttribute(da_sca_smem_kernel<512>,
                          cudaFuncAttributeMaxDynamicSharedMemorySize,
                          232448 - 1024 - 768);
-    cudaFuncSetAttribute(da_sca_smem_kernel<640>,
-                         cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         232448 - 1024 - 768);
+    smem_opt_in = true;
   }
   const size_t smem = (size_t)n_value * kE * 4 + kListBytes + 64;
   // one CTA per SM; more waves when there are many (sample, camera) pairs so
   // that each pair still splits into several CTAs
   const int waves = std::max(1, (4 * P.n_pairs + n_sm - 1) / n_sm);
-  if (threads == 640)
-    da_sca_smem_kernel<640><<<n_sm * waves, 640, smem, st>>>(P);
-  else
-    da_sca_smem_kernel<512><<<n_sm * waves, 512, smem, st>>>(P);
+  da_sca_smem_kernel<512><<<n_sm * waves, 512, smem, st>>>(P);
   return launch_status();
 }
 

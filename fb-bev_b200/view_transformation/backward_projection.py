@@ -22,13 +22,13 @@ Registry names, constructor keywords, ``forward`` signatures and state-dict
 keys match, so a FB-OCC checkpoint loads and the detector's call
 (``fbocc.py:357-363``) is unchanged.
 
-What runs where: with gradients off (inference), every nn.Linear runs on the
-Hopper tensor cores (wgmma) through ``fbbev_linear_fwd`` (3xTF32, fp32 in / out) with
-the bias, ReLU, residual add and the following LayerNorm in its epilogue; with
-gradients on they stay on cuBLAS through PyTorch (``FBBEV_TORCH_LINEAR=1`` forces
-that path).  Everything between them -- softmax, sampling-location arithmetic,
-the depth look-up, bilinear sampling, the per-camera accumulation and averaging
--- is one hand-written kernel per attention (``fbbev_msda_fused_fwd`` for the
+What runs where: every nn.Linear runs on the Hopper tensor cores (wgmma)
+through ``fbbev_linear_fwd`` (3xTF32, fp32 in / out) with the bias, ReLU,
+residual add and the following LayerNorm in its epilogue, with gradients on or
+off (``_fused_linear_on`` and ``_linear`` name the inputs that keep
+``nn.Linear``).  Everything between them -- softmax, sampling-location
+arithmetic, the depth look-up, bilinear sampling, the per-camera accumulation
+and averaging -- is one hand-written kernel per attention (``fbbev_msda_fused_fwd`` for the
 self-attention, ``fbbev_da_sca_fwd`` for the depth-aware cross-attention).  The
 reference's per-camera ``nonzero()`` loops, zero-padded re-batching, int64
 one-hot tensor and scatter loops (spatial_cross_attention_depth.py:156-216) have
@@ -36,7 +36,6 @@ no counterpart here: the kernel iterates cameras per BEV query.
 """
 import copy
 import math
-import os
 import warnings
 
 import torch
@@ -86,13 +85,9 @@ def _const_tensor(values, device):
 def _fused_linear_on(x, *dropouts):
     """The tensor-core Linear path: CUDA fp32 input, no active dropout.  With
     autograd recording the forward stays on the wgmma kernel
-    (``ops.linear.LinearTF32Function``; backward = library GEMMs) unless
-    ``FBBEV_TRAIN_TORCH_LINEAR=1`` asks for nn.Linear end to end."""
-    if os.environ.get('FBBEV_TORCH_LINEAR', '0') == '1':
-        return False
-    if torch.is_grad_enabled() and \
-            os.environ.get('FBBEV_TRAIN_TORCH_LINEAR', '0') == '1':
-        return False
+    (``ops.linear.LinearTF32Function``; backward = library GEMMs).  Callers
+    look this function up at call time, so ``oracle.gpu_ref``'s
+    ``eager_reference_mode`` can replace it to run nn.Linear throughout."""
     if not x.is_cuda or x.dtype != torch.float32:
         return False
     for d in dropouts:
@@ -138,10 +133,8 @@ def _linear(mod, x, relu=False, residual=None, norm=None):
 def _linear_pair(owner, mod_a, mod_b, x, x_add=None):
     """``(mod_a(x + x_add), mod_b(x + x_add))`` for two nn.Linears on the same
     input, one launch when their widths allow (the addition happens in the
-    kernel's loader); set ``FBBEV_LINEAR_PAIR=0`` for two launches."""
-    if (os.environ.get('FBBEV_LINEAR_PAIR', '1') == '1'
-            and mod_a.weight.shape[1] % 4 == 0
-            and not torch.is_grad_enabled()):
+    kernel's loader)."""
+    if mod_a.weight.shape[1] % 4 == 0 and not torch.is_grad_enabled():
         return _linear_ops.linear_pair(
             x, mod_a.weight, mod_a.bias, mod_b.weight, mod_b.bias,
             owner.__dict__.setdefault('_pair_cache', {}), x_add=x_add)
@@ -260,7 +253,6 @@ class FFN(BaseModule):
                 if self.add_identity else None
             fc1, fc2 = self.layers[0][0], self.layers[-2]
             if (torch.is_grad_enabled() and self.num_fcs == 2 and
-                    os.environ.get('FBBEV_FFN_FUSED', '1') == '1' and
                     _linear_ops.ffn_train_supported(x, fc1.weight, fc2.weight,
                                                     post_norm)):
                 # training on the same kernel: the backward's data path is
@@ -270,7 +262,6 @@ class FFN(BaseModule):
                     identity=identity, add_identity=self.add_identity,
                     norm=post_norm)
             if (self.num_fcs == 2 and
-                    os.environ.get('FBBEV_FFN_FUSED', '1') == '1' and
                     _linear_ops.ffn_supported(x, fc1.weight, fc2.weight) and
                     (post_norm is None or
                      _linear_ops.ln_supported(fc2.weight.shape[0]))):
@@ -892,8 +883,8 @@ class bevformer_encoder(BaseModule):
     """Encoder: builds the voxel-centre reference points, projects them into
     every camera and runs the layer stack.
 
-    ``fused_geometry`` (default True; ``FBBEV_EXACT_GEOMETRY=1`` or setting the
-    attribute to False turns it off): ``forward`` projects the reference points
+    ``fused_geometry`` (default True; setting the attribute to False turns it
+    off): ``forward`` projects the reference points
     with one kernel (``fbbev_point_sampling``) instead of ``point_sampling``'s
     ~20 eager ops (cuBLAS batched 3x3 products for 200x200x4 points x 6
     cameras).  Same fp32 chain in the same rounding order as the eager
@@ -904,9 +895,7 @@ class bevformer_encoder(BaseModule):
     test_fused_point_sampling_bit_exact), which keeps the reference's exact
     contract."""
 
-    fused_geometry = os.environ.get('FBBEV_EXACT_GEOMETRY', '0') != '1'
-    # overlap the geometry / camera-value branch with the self-attention
-    side_stream = os.environ.get('FBBEV_SIDE_STREAM', '1') == '1'
+    fused_geometry = True
 
     @staticmethod
     def _side(device):
@@ -1052,8 +1041,7 @@ class bevformer_encoder(BaseModule):
         ref_2d = cache[ck]
         if self.fused_geometry and bev_query.is_cuda:
             ref_3d = None  # only consumed by point_sampling
-            if self.side_stream and not torch.is_grad_enabled() and \
-                    bev_mask is None:
+            if not torch.is_grad_enabled() and bev_mask is None:
                 # nothing before the first cross-attention depends on the
                 # camera geometry or on the projected camera features: run
                 # them (~25 small launches + one Linear) on a side stream

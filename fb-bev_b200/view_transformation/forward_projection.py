@@ -26,8 +26,6 @@ only bit-exact if the fp32 coordinates it starts from are rounded identically
 import torch
 import torch.nn as nn
 
-import os
-
 from ..ops.bev_pool_v2 import (DeferredVolumeTrain, VoxelIndex, bev_pool_v2,
                                bev_pool_v2_deferred,
                                bev_pool_v2_dense, deferred_supported,
@@ -68,10 +66,10 @@ def gen_dx_bx(xbound, ybound, zbound):
 class _LSSBase(BaseModule):
     """Shared geometry / index machinery of the 2-D and 3-D transformers.
 
-    ``fused_geometry`` (class attribute, default True; env
-    ``FBBEV_EXACT_GEOMETRY=1`` or setting the attribute to False turns it off):
-    ``forward`` evaluates the frustum -> ego chain inside the voxelisation
-    kernel instead of materialising ``get_lidar_coor``'s (B,N,D,H,W,3) tensor
+    ``fused_geometry`` (class attribute, default True; setting the attribute
+    to False turns it off): ``forward`` evaluates the frustum -> ego chain
+    inside the voxelisation kernel instead of materialising
+    ``get_lidar_coor``'s (B,N,D,H,W,3) tensor
     through eager PyTorch (cuBLAS batched 3x3 products for 338k points, many
     times the pooling kernel).  Both routes implement the same fp32
     chain with the same rounding order (``mat3_apply_ref`` in csrc/common.cuh
@@ -81,7 +79,7 @@ class _LSSBase(BaseModule):
     the reference's exact contract.
     """
 
-    fused_geometry = os.environ.get('FBBEV_EXACT_GEOMETRY', '0') != '1'
+    fused_geometry = True
 
     def __init__(self, grid_config, input_size, downsample, accelerate,
                  uniform, with_cp):

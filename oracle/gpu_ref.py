@@ -26,7 +26,6 @@ Results tables must label this "reference (PyTorch restatement; mmcv kernel
 unavailable)".
 """
 import contextlib
-import os
 
 import torch
 import torch.nn.functional as F
@@ -177,23 +176,20 @@ def eager_reference_mode(*modules):
     ``fused_geometry`` is switched off for the duration."""
     from fbbev_b200.view_transformation import backward_projection as bp_mod
     saved = (bp_mod.ms_deform_attn_fused,
-             bp_mod.da_spatial_cross_attention_core)
-    saved_env = os.environ.get('FBBEV_TORCH_LINEAR')
+             bp_mod.da_spatial_cross_attention_core,
+             bp_mod._fused_linear_on)
     saved_geo = [(m, m.__dict__.get('fused_geometry')) for m in modules]
     bp_mod.ms_deform_attn_fused = msda_fused_eager
     bp_mod.da_spatial_cross_attention_core = da_sca_core_eager
-    os.environ['FBBEV_TORCH_LINEAR'] = '1'
+    bp_mod._fused_linear_on = lambda x, *dropouts: False
     for m in modules:
         m.fused_geometry = False
     try:
         yield
     finally:
         (bp_mod.ms_deform_attn_fused,
-         bp_mod.da_spatial_cross_attention_core) = saved
-        if saved_env is None:
-            os.environ.pop('FBBEV_TORCH_LINEAR', None)
-        else:
-            os.environ['FBBEV_TORCH_LINEAR'] = saved_env
+         bp_mod.da_spatial_cross_attention_core,
+         bp_mod._fused_linear_on) = saved
         for m, v in saved_geo:
             if v is None:
                 m.__dict__.pop('fused_geometry', None)

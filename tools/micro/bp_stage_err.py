@@ -11,6 +11,7 @@ import numpy as np
 import torch
 
 from bp_common import build_bp, cam_params
+from fbbev_b200.view_transformation import backward_projection as bp_mod
 
 DEV = "cuda:0"
 
@@ -69,11 +70,15 @@ def run(case, fused):
         out2 = bp(mlvl, None, lss_bev=t(g["lss_bev"]),
                   cam_params=cam_params(g, DEV), pred_img_depth=t(g["depth"]))
     print("  final err with golden geometry", e(out2, g["out"]))
-    os.environ['FBBEV_TORCH_LINEAR'] = '1'
-    with torch.no_grad():
-        out3 = bp(mlvl, None, lss_bev=t(g["lss_bev"]),
-                  cam_params=cam_params(g, DEV), pred_img_depth=t(g["depth"]))
-    os.environ['FBBEV_TORCH_LINEAR'] = '0'
+    fused_linear_on = bp_mod._fused_linear_on
+    bp_mod._fused_linear_on = lambda x, *dropouts: False
+    try:
+        with torch.no_grad():
+            out3 = bp(mlvl, None, lss_bev=t(g["lss_bev"]),
+                      cam_params=cam_params(g, DEV),
+                      pred_img_depth=t(g["depth"]))
+    finally:
+        bp_mod._fused_linear_on = fused_linear_on
     print("  ... and torch Linears", e(out3, g["out"]))
     print("  |out| max", float(np.abs(g["out"]).max()))
 
