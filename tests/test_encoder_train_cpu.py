@@ -253,9 +253,9 @@ def _check(text, entries, names):
 def test_ffn_training_instantiations():
     """kTrainFwd (1) and kBwd (2) for every (pad16(E), K-blocks) the
     inference kernel has."""
+    from test_ffn_ptxas import ffn_instantiations
     text, entries = _entries("ffn_tf32")
-    want = {(a, b, mode) for a, b in
-            {(16, 1), (32, 1), (48, 1), (48, 2), (64, 2), (80, 2)} for mode in (1, 2)}
+    want = {t for t in ffn_instantiations() if t[2] > 0}
     found = {}
     for fn in entries:
         m = re.search(r"ffn_tf32_kernelILi(\d+)ELi(\d+)ELi(\d+)E", fn)
