@@ -4,9 +4,8 @@
 #include <stdint.h>
 
 namespace fbbev {
-namespace bulk {
 
-__device__ __forceinline__ uint32_t smem_addr(const void* p) {
+__device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -20,6 +19,10 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t tx)
                "r"(tx)
                : "memory");
 }
+// Spins until the phase of `bar` with `parity` has completed.  A kernel that
+// issues wgmma instantiates it with DRAIN_WGMMA: the trap path then waits for
+// the warpgroup's MMAs itself (ptxas would inject that wait, C7517).
+template <bool DRAIN_WGMMA = false>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t done = 0;
   for (uint32_t spins = 0; !done; ++spins) {
@@ -30,7 +33,10 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "=r"(done)
         : "r"(bar), "r"(parity)
         : "memory");
-    if (spins > (1u << 26)) __trap();  // a protocol bug must not hang the GPU
+    if (spins > (1u << 26)) {  // a protocol bug must not hang the GPU
+      if (DRAIN_WGMMA) asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(0) : "memory");
+      __trap();
+    }
   }
 }
 // non-blocking probe of a phase
@@ -45,10 +51,10 @@ __device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
       : "memory");
   return done != 0;
 }
-// global -> shared, `bytes` a multiple of 16, both addresses 16-byte aligned;
-// completion is signalled on `bar` as transaction bytes
-__device__ __forceinline__ void g2s(uint32_t dst, const void* src, uint32_t bytes,
-                                    uint32_t bar) {
+// global -> shared 1-D bulk copy (TMA): `bytes` a multiple of 16, both
+// addresses 16-byte aligned; completion is signalled on `bar` as tx bytes
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src,
+                                         uint32_t bytes, uint32_t bar) {
   asm volatile(
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes "
       "[%0], [%1], %2, [%3];" ::"r"(dst),
@@ -64,11 +70,10 @@ __device__ __forceinline__ float2 ld2(const float* p) {
     float2 v;
     asm("ld.shared.v2.f32 {%0, %1}, [%2];"
         : "=f"(v.x), "=f"(v.y)
-        : "r"(smem_addr(p)));
+        : "r"(smem_u32(p)));
     return v;
   }
   return __ldg(reinterpret_cast<const float2*>(p));
 }
 
-}  // namespace bulk
 }  // namespace fbbev

@@ -118,8 +118,8 @@ __device__ __forceinline__ void sample_map(const float* map, int H, int W,
   const float* p4 = map + (h1 * W + x1) * kE;
 #pragma unroll
   for (int c = 0; c < kCH / 2; ++c) {
-    const float2 v1 = bulk::ld2<SMEM>(p1 + 2 * c), v2 = bulk::ld2<SMEM>(p2 + 2 * c);
-    const float2 v3 = bulk::ld2<SMEM>(p3 + 2 * c), v4 = bulk::ld2<SMEM>(p4 + 2 * c);
+    const float2 v1 = ld2<SMEM>(p1 + 2 * c), v2 = ld2<SMEM>(p2 + 2 * c);
+    const float2 v3 = ld2<SMEM>(p3 + 2 * c), v4 = ld2<SMEM>(p4 + 2 * c);
     // same association as sample_accum: (w1 v1 + w2 v2 + w3 v3 + w4 v4) * wgt
     const float sx = w1 * v1.x + w2 * v2.x + w3 * v3.x + w4 * v4.x;
     const float sy = w1 * v1.y + w2 * v2.y + w3 * v3.y + w4 * v4.y;
@@ -201,7 +201,7 @@ __device__ __forceinline__ void sca_pass(const ScaSmemParams& P, const ScaCtx& C
   for (int z = 0; z < kZ; ++z) dw[z] = __shfl_sync(kFull, dwz, (lane & ~7) | z);
   // the staged map is used as soon as its bulk copies have landed; until then
   // (the first ~10 us of the CTA) the same gathers go to the global original
-  if (!tile_ready) tile_ready = bulk::mbar_test(bulk::smem_addr(C.bar), 0);
+  if (!tile_ready) tile_ready = mbar_test(smem_u32(C.bar), 0);
   if (active) {
 #pragma unroll
     for (int p = 0; p < kPts; ++p) {          // point index = pp * Z + z (:563-570)
@@ -249,8 +249,8 @@ __global__ void __launch_bounds__(kScaThreads, 1) da_sca_smem_kernel(
   const long long spare = (long long)gridDim.x - P.n_pairs;
   if (threadIdx.x == 0) {
     s_total = 0; s_next = 0; s_left_n = 0; s_pair = -1;
-    bulk::mbar_init(bulk::smem_addr(bar), 1);
-    bulk::fence_mbar_init();
+    mbar_init(smem_u32(bar), 1);
+    fence_mbar_init();
   }
   __syncthreads();
   {  // total of all partial counts
@@ -296,11 +296,11 @@ __global__ void __launch_bounds__(kScaThreads, 1) da_sca_smem_kernel(
   const int bn = pair;                        // value / depth are (b, n) major
 
   if (threadIdx.x == 0) {
-    const uint32_t barrier = bulk::smem_addr(bar);
-    bulk::mbar_arrive_expect_tx(barrier, (uint32_t)tile_bytes);
+    const uint32_t barrier = smem_u32(bar);
+    mbar_arrive_expect_tx(barrier, (uint32_t)tile_bytes);
     const char* src = reinterpret_cast<const char*>(
         P.value + (int64_t)bn * P.n_value * kE);
-    const uint32_t dst = bulk::smem_addr(tile);
+    const uint32_t dst = smem_u32(tile);
     // the K CTAs of a camera all pull the same 225 KB: start each one at a
     // different chunk so that they do not queue on the same L2 lines
     constexpr int kChunk = 8192;
@@ -309,7 +309,7 @@ __global__ void __launch_bounds__(kScaThreads, 1) da_sca_smem_kernel(
     for (int c = 0; c < n_chunks; ++c) {
       const int off = ((start + c) % n_chunks) * kChunk;
       const int nb = min(kChunk, tile_bytes - off);
-      bulk::g2s(dst + off, src + off, (uint32_t)nb, barrier);
+      bulk_g2s(dst + off, src + off, (uint32_t)nb, barrier);
     }
   }
 
@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(kScaThreads, 1) da_sca_smem_kernel(
   }
   // the bulk copies must have landed before the CTA (and its shared memory)
   // goes away, also when this warp never touched the tile
-  if (!tile_ready) bulk::mbar_wait(bulk::smem_addr(bar), 0);
+  if (!tile_ready) mbar_wait(smem_u32(bar), 0);
 }
 
 size_t da_sca_smem_workspace_bytes(int bs, int n_cams) {

@@ -78,11 +78,8 @@
 namespace fbbev {
 namespace ffn {
 
-constexpr int kTileM = 128;
+constexpr int kTileM = kATileM;
 constexpr int kUnitM = 64;              // rows per warpgroup and step
-constexpr int kAPart = kTileM * kKB * 4;            // bytes of A_hi (== A_lo)
-constexpr int kABlock = 2 * kAPart;                 // one K-block, hi + lo
-constexpr int kAChunkStride = (kTileM / 8) * 128;   // bytes between K chunks
 constexpr int kThreads = 256;           // two warpgroups
 constexpr int kWarps = kThreads / 32;
 constexpr int kHC = 80;                 // hidden columns per GEMM1 chunk
@@ -90,7 +87,7 @@ constexpr int kMaxE = 80;
 constexpr int kMaxHidden = 320;
 constexpr int kXPitch = 84;             // floats per X row: conflict-free fragment loads
 constexpr int kSlots = 4;
-constexpr int kWStage = 2 * kHC * kKB * 4;          // >= 2 * pad16(E) * kKB * 4
+constexpr int kWStage = 2 * kb_part(kHC);          // >= 2 * kb_part(pad16(E))
 constexpr int kXBytes = kTileM * kXPitch * 4;
 constexpr int kHBytes = (kHC / kKB) * kABlock;
 constexpr int kBarBytes = 8 * (kSlots + kWarps) + 4 * kSlots + 16;
@@ -126,12 +123,6 @@ struct TrainParams : Params {
 };
 template <int MODE> struct ParamsFor { using type = TrainParams; };
 template <> struct ParamsFor<kInfer> { using type = Params; };
-
-// A-tile offset (bytes) of element (row, col) of a [128 x 40 k] block image
-__device__ __forceinline__ uint32_t a_off(int row, int col) {
-  return (uint32_t)((col >> 2) * (kTileM / 8) + (row >> 3)) * 128u + (row & 7) * 16u +
-         (col & 3) * 4u;
-}
 
 __device__ __forceinline__ void bar_sync_wg(int wg) {
   asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
@@ -301,7 +292,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       bytes = kWStage;
     } else {
       src = p.w2p + (size_t)(c * (kHC / kKB) + t - KB1) * (2 * NP2 * kKB);
-      bytes = 2u * NP2 * kKB * 4u;
+      bytes = 2u * kb_part(NP2);
     }
     const uint32_t s = i % kSlots;
     mbar_arrive_expect_tx(full + 8u * s, bytes);
@@ -312,7 +303,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 
   int it = 0;   // next stage to consume
   int rel = 0;  // next stage to release
-  auto wait_stage = [&]() { mbar_wait(full + 8u * (it % kSlots), (it / kSlots) & 1u); };
+  auto wait_stage = [&]() { mbar_wait<true>(full + 8u * (it % kSlots), (it / kSlots) & 1u); };
   // the warp's MMAs on stages [rel, rel + n) have drained: arrive; the eighth
   // arrival refills the slot
   auto release = [&](int n) {
@@ -353,16 +344,13 @@ __global__ void __launch_bounds__(kThreads, 1)
   const int my_steps = my_chunks / n_hc;
   auto frag = [&](uint32_t (&fh)[kKSteps][4], uint32_t (&fl)[kKSteps][4], int kb, int gg) {
     const int s = gg / n_hc, c = gg - s * n_hc;
-    if (kb == 0 && c == 0) mbar_wait(xb, s & 1);
+    if (kb == 0 && c == 0) mbar_wait<true>(xb, s & 1);
 #pragma unroll
     for (int k = 0; k < kKSteps; ++k)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int r = (lane >> 2) + 8 * (e & 1), col = kb * kKB + 8 * k + q + 4 * (e >> 1);
-        const float v = xw[r * kXPitch + col];
-        const float hi = tf32_hi(v);
-        fh[k][e] = __float_as_uint(hi);
-        fl[k][e] = __float_as_uint(v - hi);
+        tf32_split(xw[r * kXPitch + col], fh[k][e], fl[k][e]);
       }
     if (kb == KB1 - 1 && c == n_hc - 1 && s + 1 < my_steps) fill_x(s + 1);
   };
@@ -372,15 +360,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     wait_stage();
     const uint32_t w_hi = ws_a + (it % kSlots) * kWStage;
     wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < kKSteps; ++k) {
-      const uint32_t b = w_hi + 2u * k * (kHC * 16);
-      const uint64_t dbh = smem_desc(b, kHC * 16, 128);
-      const uint64_t dbl = smem_desc(b + kHC * kKB * 4, kHC * 16, 128);
-      wgmma_tf32_rs<kHC>(acc, fh[k], dbh, kb > 0 || k > 0);
-      wgmma_tf32_rs<kHC>(acc, fl[k], dbh, 1u);
-      wgmma_tf32_rs<kHC>(acc, fh[k], dbl, 1u);
-    }
+    wg_kblock_3xtf32_rs<kHC>(acc, fh, fl, w_hi, w_hi + kb_part(kHC), kb_chunk(kHC), kb > 0);
     ++it;
     wgmma_commit();
   };
@@ -447,11 +427,9 @@ __global__ void __launch_bounds__(kThreads, 1)
             v = fmaxf(v, 0.f);
           }
           vv[e] = v;
-          const float hi = tf32_hi(v);
           unsigned char* a = h_base + (J / kKSteps) * kABlock +
                              (J % kKSteps) * 2 * kAChunkStride + h * 128 + e * 4;
-          *reinterpret_cast<float*>(a) = hi;
-          *reinterpret_cast<float*>(a + kAPart) = v - hi;
+          tf32_split(v, *reinterpret_cast<float*>(a), *reinterpret_cast<float*>(a + kAPart));
         }
         if constexpr (MODE != kInfer) {
           if (hrow + 8 * h < p.M)
@@ -473,7 +451,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       const uint32_t w_hi = ws_a + (it % kSlots) * kWStage;
       wgmma_fence();
       wg_kblock_3xtf32<NP2>(acc2, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
-                            w_hi + NP2 * kKB * 4, NP2 * 16, c > 0 || j > 0);
+                            w_hi + kb_part(NP2), kb_chunk(NP2), c > 0 || j > 0);
       ++it;
     }
     wgmma_commit();

@@ -48,14 +48,11 @@ namespace fbbev {
 namespace hfuse {
 
 constexpr int kThreads = 256;        // two warpgroups
-constexpr int kTileM = 128;
+constexpr int kTileM = kATileM;
 constexpr int kMaxC = 80;            // GEMM1 width (Wt' rows padded to 80)
 constexpr int kHalf = 80;            // GEMM2 columns per half
 constexpr int kMaxCout = 2 * kHalf;
-constexpr int kAPart = kTileM * kKB * 4;           // bytes of H_hi (== H_lo) per K-block
-constexpr int kABlock = 2 * kAPart;
-constexpr int kAChunkStride = (kTileM / 8) * 128;  // bytes between K chunks of H
-constexpr int kWPart = kHalf * kKB * 4;            // bytes of one hi / lo part of a stage
+constexpr int kWPart = kb_part(kHalf);             // bytes of one hi / lo part of a stage
 constexpr int kWStage = 2 * kWPart;                // 25.6 KB
 constexpr int kCv = 2 * kMaxC + kMaxCout;          // bias_t | time_w | bias_c
 // shared memory: Wt' | H tile | weight ring | corner table | constants | mbarriers
@@ -83,12 +80,6 @@ struct Params {
   int64_t curr_bstride, hist_bstride, next_bstride;
   int T, C, Cout, Z, H, W, zhw, n_kb, tps, n_tiles;
 };
-
-// H-tile offset (bytes) of element (row, col) of a [128 x 40 k] block image
-__device__ __forceinline__ uint32_t a_off(int row, int col) {
-  return (uint32_t)((col >> 2) * (kTileM / 8) + (row >> 3)) * 128u + (row & 7) * 16u +
-         (col & 3) * 4u;
-}
 
 __device__ __forceinline__ bool is_fresh(const Params& p, int b) {
   return !p.hist || __ldg(p.fresh + b) != 0;
@@ -158,7 +149,7 @@ __global__ void __launch_bounds__(kThreads, 1) history_fuse_kernel(const Params 
   }
   issue_w();
   issue_w();
-  mbar_wait(bar_wt, 0);
+  mbar_wait<true>(bar_wt, 0);
 
   const int rl = wg * 64 + wq * 16 + (lane >> 2);  // tile row of acc[.. + 0 / 1]
   uint32_t it = 0;
@@ -243,21 +234,10 @@ __global__ void __launch_bounds__(kThreads, 1) history_fuse_kernel(const Params 
 #pragma unroll
         for (int k = 0; k < kKSteps; ++k)
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float hi = tf32_hi(a[k][e]);
-            ah[k][e] = __float_as_uint(hi);
-            al[k][e] = __float_as_uint(a[k][e] - hi);
-          }
+          for (int e = 0; e < 4; ++e) tf32_split(a[k][e], ah[k][e], al[k][e]);
         wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < kKSteps; ++k) {
-          const uint32_t b_hi = wt_a + kb * kWStage + 2u * k * kMaxC * 16u;
-          const uint64_t dbh = smem_desc(b_hi, kMaxC * 16, 128);
-          const uint64_t dbl = smem_desc(b_hi + kWPart, kMaxC * 16, 128);
-          wgmma_tf32_rs<kMaxC>(acc1, ah[k], dbh, kb > 0 || k > 0);
-          wgmma_tf32_rs<kMaxC>(acc1, al[k], dbh, 1u);
-          wgmma_tf32_rs<kMaxC>(acc1, ah[k], dbl, 1u);
-        }
+        const uint32_t b_hi = wt_a + kb * kWStage;
+        wg_kblock_3xtf32_rs<kMaxC>(acc1, ah, al, b_hi, b_hi + kWPart, kb_chunk(kMaxC), kb > 0);
         wgmma_commit();
         // also drains the previous frame's GEMM2: the H tile is free after this
         wgmma_wait<0>();
@@ -273,10 +253,8 @@ __global__ void __launch_bounds__(kThreads, 1) history_fuse_kernel(const Params 
           for (int e = 0; e < 2; ++e) {
             const int col = 8 * J + 2 * q + e;
             const float v = fmaxf(acc1[4 * J + 2 * h + e] + fmaf(time_w[col], st, bias_t[col]), 0.f);
-            const float hi = tf32_hi(v);
             unsigned char* d = hs + (size_t)(col / kKB) * kABlock + a_off(rl + 8 * h, col % kKB);
-            *reinterpret_cast<float*>(d) = hi;
-            *reinterpret_cast<float*>(d + kAPart) = v - hi;
+            tf32_split(v, *reinterpret_cast<float*>(d), *reinterpret_cast<float*>(d + kAPart));
           }
         }
       }
@@ -286,12 +264,12 @@ __global__ void __launch_bounds__(kThreads, 1) history_fuse_kernel(const Params 
       for (int h = 0; h < NH; ++h) {
         for (int kb = 0; kb < n_kb; ++kb) {
           const uint32_t sl = it & 1;
-          mbar_wait(bar + 8u * sl, (it >> 1) & 1u);
+          mbar_wait<true>(bar + 8u * sl, (it >> 1) & 1u);
           const uint32_t a_hi = hs_a + kb * kABlock + wg * 1024u;
           const uint32_t w_hi = ws_a + sl * kWStage;
           wgmma_fence();
           wg_kblock_3xtf32<kHalf>(acc2[h], a_hi, a_hi + kAPart, kAChunkStride, w_hi,
-                                  w_hi + kWPart, kHalf * 16, s > 0 || kb > 0);
+                                  w_hi + kWPart, kb_chunk(kHalf), s > 0 || kb > 0);
           // once the previous stage's MMAs have drained (both warpgroups), its
           // slot takes the stage after this one
           wgmma_commit();

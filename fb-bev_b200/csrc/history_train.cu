@@ -91,7 +91,7 @@ __device__ __forceinline__ double warp_rows_sum(double v) {
 template <int N, int EPI>
 __global__ void __launch_bounds__(kThreads, 1) history_train_gemm_kernel(const Params p) {
   extern __shared__ __align__(128) unsigned char smem[];
-  const int kb_bytes = 2 * kKB * N * 4;
+  const int kb_bytes = 2 * kb_part(N);
   const int w_bytes = p.n_seg * p.n_kb * kb_bytes;
   const uint32_t w_a = smem_u32(smem);
   float* cv = reinterpret_cast<float*>(smem + w_bytes);
@@ -136,7 +136,7 @@ __global__ void __launch_bounds__(kThreads, 1) history_train_gemm_kernel(const P
   const float* gamma = cv + 4 * kCvLen;
   const float* beta = cv + 5 * kCvLen;
   double* red_w = red + warp * 2 * kMaxC;
-  mbar_wait(bar, 0);
+  mbar_wait<true>(bar, 0);
 
   const int rl = wg * 64 + wq * 16 + (lane >> 2);  // tile row of acc[.. + 0 / 1]
   for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
@@ -157,21 +157,12 @@ __global__ void __launch_bounds__(kThreads, 1) history_train_gemm_kernel(const P
             const int c = kb * kKB + 8 * k + q + 4 * (e >> 1);
             const float v =
                 c < p.k_seg ? __ldg(base + (int64_t)c * zhw + ((e & 1) ? vr1 : vr0)) : 0.f;
-            const float hi = tf32_hi(v);
-            ah[k][e] = __float_as_uint(hi);
-            al[k][e] = __float_as_uint(v - hi);
+            tf32_split(v, ah[k][e], al[k][e]);
           }
         wgmma_fence();
         const uint32_t b_kb = w_a + (uint32_t)((s * p.n_kb + kb) * kb_bytes);
-#pragma unroll
-        for (int k = 0; k < kKSteps; ++k) {
-          const uint32_t b_hi = b_kb + 2u * k * N * 16u;
-          const uint64_t dbh = smem_desc(b_hi, N * 16, 128);
-          const uint64_t dbl = smem_desc(b_hi + N * kKB * 4, N * 16, 128);
-          wgmma_tf32_rs<N>(acc, ah[k], dbh, (s | kb | k) != 0);
-          wgmma_tf32_rs<N>(acc, al[k], dbh, 1u);
-          wgmma_tf32_rs<N>(acc, ah[k], dbl, 1u);
-        }
+        wg_kblock_3xtf32_rs<N>(acc, ah, al, b_kb, b_kb + kb_part(N), kb_chunk(N),
+                               (s | kb) != 0);
         wgmma_commit();
         wgmma_wait<0>();
       }
@@ -401,7 +392,7 @@ static int launch_gemm(const Params& p, int frames, cudaStream_t st, int* grid =
   // thing the shared memory depends on; n_seg * n_kb <= 2 * 4)
   static int resident[9] = {};
   const int blocks = p.n_seg * p.n_kb;
-  const int smem = blocks * 2 * kKB * N * 4 + kNumCv * kCvLen * 4 + kRedBytes + 16;
+  const int smem = blocks * 2 * kb_part(N) + kNumCv * kCvLen * 4 + kRedBytes + 16;
   if (blocks > 8 || smem > kSmemLimit) return FBBEV_ERR_UNSUPPORTED;
   if (!resident[blocks]) {
     cudaError_t e =

@@ -40,9 +40,7 @@
 namespace fbbev {
 
 constexpr int kChunks = kKB / 4;                 // 16-byte chunks per row
-constexpr int kTileM = 128;
-constexpr int kAPart = kTileM * kKB * 4;         // bytes of A_hi (== A_lo)
-constexpr int kAChunkStride = (kTileM / 8) * 128;  // bytes between K chunks
+constexpr int kTileM = kATileM;
 constexpr int kLinThreads = 256;                 // two warpgroups
 constexpr int kMaxN = 192;
 constexpr int kMaxLnN = 80;  // widest LayerNorm row (the encoder's embed_dims)
@@ -64,8 +62,7 @@ __global__ void linear_pack_kernel(const float* __restrict__ w, int n, int k,
     for (int j = 0; j < 4; ++j) {
       const int col = kb * kKB + ch * 4 + j;
       const float v = (row < n && col < k) ? w[(int64_t)row * k + col] : 0.f;
-      hi[j] = tf32_hi(v);
-      lo[j] = v - hi[j];
+      tf32_split(v, hi[j], lo[j]);
     }
     const int64_t part = (int64_t)kChunks * npad * 4;  // floats of one hi / lo part
     const int64_t off =
@@ -209,7 +206,7 @@ template <int NPAD, bool LN, bool STATS>
 __global__ void __launch_bounds__(kLinThreads, 1)
     linear_tf32_kernel(const LinearParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
-  constexpr uint32_t w_part = NPAD * kKB * 4;              // bytes of W_hi
+  constexpr uint32_t w_part = kb_part(NPAD);              // bytes of W_hi
   constexpr uint32_t stage_bytes = 2u * kAPart + 2u * w_part;
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
@@ -275,9 +272,11 @@ __global__ void __launch_bounds__(kLinThreads, 1)
       const int r = idx / kChunks, ch = idx - r * kChunks;
       const float4 x = v[i];
       float4 hi, lo;
-      hi.x = tf32_hi(x.x); hi.y = tf32_hi(x.y); hi.z = tf32_hi(x.z); hi.w = tf32_hi(x.w);
-      lo.x = x.x - hi.x; lo.y = x.y - hi.y; lo.z = x.z - hi.z; lo.w = x.w - hi.w;
-      const uint32_t off = (uint32_t)(ch * (kTileM / 8) + (r >> 3)) * 128u + (r & 7) * 16u;
+      tf32_split(x.x, hi.x, lo.x);
+      tf32_split(x.y, hi.y, lo.y);
+      tf32_split(x.z, hi.z, lo.z);
+      tf32_split(x.w, hi.w, lo.w);
+      const uint32_t off = a_off(r, 4 * ch);
       *reinterpret_cast<float4*>(a_st + off) = hi;
       *reinterpret_cast<float4*>(a_st + off + kAPart) = lo;
     }
@@ -295,12 +294,12 @@ __global__ void __launch_bounds__(kLinThreads, 1)
   int kb = 0, tile = blockIdx.x;
   for (int g = 0; g < n_steps; ++g) {
     const uint32_t s = g & 1;
-    mbar_wait(bar + 8u * s, (g >> 1) & 1u);
+    mbar_wait<true>(bar + 8u * s, (g >> 1) & 1u);
     const uint32_t a_hi = smem_base + s * stage_bytes + wg * 1024u;  // 8 row groups
     const uint32_t w_hi = smem_base + s * stage_bytes + 2u * kAPart;
     wgmma_fence();
     wg_kblock_3xtf32<NPAD>(acc, a_hi, a_hi + kAPart, kAChunkStride, w_hi,
-                           w_hi + w_part, NPAD * 16, kb > 0);
+                           w_hi + w_part, kb_chunk(NPAD), kb > 0);
     wgmma_commit();
     // step g - 1's MMAs (both warpgroups) have read stage s ^ 1: refill it
     // with step g + 1 while step g's MMAs run, and start the loads of g + 2
@@ -343,8 +342,8 @@ __global__ void __launch_bounds__(kLinThreads, 1)
 // barrier: the warp refills it as soon as it has read it -- right after the A
 // fragments are in registers when there is no residual, after the epilogue
 // otherwise.  The A operand is formed in registers: x (+ x_add, one fp32 add
-// as torch), hi = tf32_hi, lo = x - hi, and the same three MMAs per k8 step
-// as wg_kblock_3xtf32, in the same order.  X rows have a pitch of 84 floats,
+// as torch), split hi / lo, and the same three MMAs per k8 step as
+// wg_kblock_3xtf32 (wg_kblock_3xtf32_rs).  X rows have a pitch of 84 floats,
 // which makes the fragment loads free of bank conflicts; residual rows have
 // NPAD + 8 (conflict-free float2 loads).
 constexpr int kRTileM = 64;
@@ -354,42 +353,33 @@ constexpr int kMaxStages = 4;
 constexpr int kSmemLimit = 227 * 1024;  // opt-in shared memory per CTA (sm_90)
 
 template <int NPAD>
-constexpr uint32_t resident_w_bytes() { return 2u * 2u * NPAD * kKB * 4u; }
+constexpr uint32_t resident_w_bytes() { return 2u * 2u * kb_part(NPAD); }
 
 // The MMAs of one 64-row tile over its two K-blocks, A from the raw stage in
-// registers: v = x + x_add (one fp32 add), hi = tf32_hi(v), lo = v - hi,
-// columns >= K zero; per k8 step the three products of wg_kblock_3xtf32 in
-// its order.  A K-block's fragments are formed before its fence, so the next
-// block's shared-memory loads overlap the MMAs of this one.
+// registers: v = x + x_add (one fp32 add), split hi / lo, columns >= K zero.
+// A K-block's fragments are formed before its fence, so the next block's
+// shared-memory loads overlap the MMAs of this one.
 template <int NPAD>
 __device__ __forceinline__ void resident_mma(float (&acc)[NPAD / 2], const float* xs,
                                              const float* xa, int xa_pitch, int rl, int q,
                                              int K, uint32_t w_base) {
-  constexpr uint32_t w_part = NPAD * kKB * 4;
-  uint32_t a_hi[2 * kKSteps][4], a_lo[2 * kKSteps][4];
+  constexpr uint32_t w_part = kb_part(NPAD);
+  uint32_t a_hi[2][kKSteps][4], a_lo[2][kKSteps][4];
 #pragma unroll
   for (int kb = 0; kb < 2; ++kb) {
 #pragma unroll
-    for (int k = kb * kKSteps; k < (kb + 1) * kKSteps; ++k)
+    for (int k = 0; k < kKSteps; ++k)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const int r = rl + 8 * (e & 1), c = 8 * k + q + 4 * (e >> 1);
+        const int r = rl + 8 * (e & 1), c = kb * kKB + 8 * k + q + 4 * (e >> 1);
         float v = __fadd_rn(xs[r * kXPitch + c], xa[r * xa_pitch + c]);
         v = c < K ? v : 0.f;
-        const float hi = tf32_hi(v);
-        a_hi[k][e] = __float_as_uint(hi);
-        a_lo[k][e] = __float_as_uint(v - hi);
+        tf32_split(v, a_hi[kb][k][e], a_lo[kb][k][e]);
       }
     wgmma_fence();
-#pragma unroll
-    for (int k = kb * kKSteps; k < (kb + 1) * kKSteps; ++k) {
-      const uint32_t b_hi = w_base + kb * 2u * w_part + 2u * (k - kb * kKSteps) * NPAD * 16u;
-      const uint64_t dbh = smem_desc(b_hi, NPAD * 16, 128);
-      const uint64_t dbl = smem_desc(b_hi + w_part, NPAD * 16, 128);
-      wgmma_tf32_rs<NPAD>(acc, a_hi[k], dbh, k > 0);
-      wgmma_tf32_rs<NPAD>(acc, a_lo[k], dbh, 1u);
-      wgmma_tf32_rs<NPAD>(acc, a_hi[k], dbl, 1u);
-    }
+    const uint32_t b_hi = w_base + kb * 2u * w_part;
+    wg_kblock_3xtf32_rs<NPAD>(acc, a_hi[kb], a_lo[kb], b_hi, b_hi + w_part, kb_chunk(NPAD),
+                              kb > 0);
   }
 }
 
@@ -397,7 +387,6 @@ template <int NPAD, bool LN, bool STATS>
 __global__ void __launch_bounds__(kLinThreads, 1)
     linear_tf32_kernel_resident(const LinearParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
-  constexpr uint32_t w_part = NPAD * kKB * 4;  // bytes of one K-block's W_hi
   constexpr int kResPitch = NPAD + 8;
   const int tid = threadIdx.x;
   const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
@@ -458,7 +447,7 @@ __global__ void __launch_bounds__(kLinThreads, 1)
     }
   };
   for (int i = 0; i < S; ++i) fill(i);
-  mbar_wait(bars, 0);
+  mbar_wait<true>(bars, 0);
 
   const int rl = 16 * wq + (lane >> 2);  // stage row of acc[.. + 0 / 1]
   const int q = lane & 3;
@@ -466,7 +455,7 @@ __global__ void __launch_bounds__(kLinThreads, 1)
   float acc[NPAD / 2];  // written first by a scale-d = 0 MMA, never zeroed
   for (int i = 0; i < n_it; ++i) {
     const int s = i % S;
-    mbar_wait(warp_bar + 32u * s, (uint32_t)(i / S) & 1u);
+    mbar_wait<true>(warp_bar + 32u * s, (uint32_t)(i / S) & 1u);
     const unsigned char* st = ring + s * p.stage_bytes;
     const float* xs = reinterpret_cast<const float*>(st);
     // no x_add: add the row of -0 (x + -0 == x for every x), so the loads
@@ -500,7 +489,7 @@ static int resident_layout(LinearParams& p, int npad) {
   p.xa_off = x_rows;
   p.res_off = p.x_add ? 2 * x_rows : x_rows;
   p.stage_bytes = p.res_off + (p.residual ? kRTileM * (npad + 8) * 4 : 0);
-  const int fixed = 2 * 2 * npad * kKB * 4 + 8 * (1 + 8 * kMaxStages) +
+  const int fixed = 2 * 2 * kb_part(npad) + 8 * (1 + 8 * kMaxStages) +
                     (3 * npad + kMaxResidentK) * 4;
   const int s = (kSmemLimit - fixed) / (2 * (int)p.stage_bytes);
   return s < kMaxStages ? s : kMaxStages;
@@ -525,7 +514,7 @@ static int launch_linear_t(const LinearParams& p, cudaStream_t st) {
     return launch_status();
   }
   constexpr size_t smem =
-      2 * (2 * (size_t)kAPart + 2 * (size_t)NPAD * kKB * 4) + 16 + 3 * NPAD * 4;
+      2 * (2 * (size_t)kAPart + 2 * (size_t)kb_part(NPAD)) + 16 + 3 * NPAD * 4;
   static int resident = 0;  // CTAs that fit on the device at once
   auto kern = linear_tf32_kernel<NPAD, LN, STATS>;
   if (!resident) {

@@ -61,10 +61,10 @@ __device__ __forceinline__ void gather_accum(const Bilinear& bl, const float* p1
   const bool ok3 = SMEM || bl.ok3(H, W), ok4 = SMEM || bl.ok4(H, W);
 #pragma unroll
   for (int c = 0; c < kCH; c += 2) {
-    const float2 v1 = ok1 ? bulk::ld2<SMEM>(p1 + c) : zero;
-    const float2 v2 = ok2 ? bulk::ld2<SMEM>(p2 + c) : zero;
-    const float2 v3 = ok3 ? bulk::ld2<SMEM>(p3 + c) : zero;
-    const float2 v4 = ok4 ? bulk::ld2<SMEM>(p4 + c) : zero;
+    const float2 v1 = ok1 ? ld2<SMEM>(p1 + c) : zero;
+    const float2 v2 = ok2 ? ld2<SMEM>(p2 + c) : zero;
+    const float2 v3 = ok3 ? ld2<SMEM>(p3 + c) : zero;
+    const float2 v4 = ok4 ? ld2<SMEM>(p4 + c) : zero;
     acc[c] += bl.blend(v1.x, v2.x, v3.x, v4.x) * wgt;
     acc[c + 1] += bl.blend(v1.y, v2.y, v3.y, v4.y) * wgt;
   }
@@ -86,19 +86,19 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) msda_self_smem_kernel(
   const float* vmap = value + (int64_t)blockIdx.z * nq * kE;
 
   if (threadIdx.x == 0) {
-    bulk::mbar_init(bulk::smem_addr(&bar), 1);
-    bulk::fence_mbar_init();
+    mbar_init(smem_u32(&bar), 1);
+    fence_mbar_init();
   }
   __syncthreads();
   if (threadIdx.x < 32) {
     if (threadIdx.x == 0)
-      bulk::mbar_arrive_expect_tx(bulk::smem_addr(&bar), kTileBytes);
+      mbar_arrive_expect_tx(smem_u32(&bar), kTileBytes);
     __syncwarp();
     // a window row is a contiguous run of kWx pixels of the map
     if (threadIdx.x < kWy)
-      bulk::g2s(bulk::smem_addr(tile + threadIdx.x * kWx * kE),
-                vmap + ((int64_t)(y0 + threadIdx.x) * W + x0) * kE, kWx * kE * 4,
-                bulk::smem_addr(&bar));
+      bulk_g2s(smem_u32(tile + threadIdx.x * kWx * kE),
+               vmap + ((int64_t)(y0 + threadIdx.x) * W + x0) * kE, kWx * kE * 4,
+               smem_u32(&bar));
   }
 
   const int m = threadIdx.x & 7, ql = threadIdx.x >> 3;
@@ -147,7 +147,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) msda_self_smem_kernel(
   for (int c = 0; c < kCH; ++c) acc[c] = 0.f;
   const float* smap = tile + m * kCH;
   const float* gmap = vmap + m * kCH;
-  bulk::mbar_wait(bulk::smem_addr(&bar), 0);
+  mbar_wait(smem_u32(&bar), 0);
 #pragma unroll
   for (int p = 0; p < kPts; ++p) {
     // NaN and +-inf locations fail this test as in the global kernels; past
