@@ -29,9 +29,6 @@ _SIGNATURES = {
     "fbbev_bev_pool_v2_fwd": (ctypes.c_int, [_p] * 7 + [_i32, _i32, _p, _p]),
     "fbbev_bev_pool_v2_dense_workspace_bytes": (
         _sz, [_i32, _i64, _i32, _i32, _i32]),
-    "fbbev_bev_pool_v2_fwd_dense": (
-        ctypes.c_int,
-        [_p] * 7 + [_i32, _p, _i32, _i32, _i32, _i64, _p, _p, _sz, _p]),
     "fbbev_bev_pool_v2_plan": (
         ctypes.c_int,
         [_p, _p, _p, _i32, _p, _i32, _i32, _i32, _i64, _p, _sz, _p]),
@@ -62,16 +59,9 @@ _SIGNATURES = {
                                   _p, _p, _p]),
     "fbbev_voxel_prepare_workspace_bytes": (_sz, [_i64, _i64]),
     "fbbev_voxel_prepare": (
-        ctypes.c_int, [_p] + [_i32] * 5 + [_p] * 3 + [_p] * 6 +
-        [_p, _sz, _i32, _p, _sz, _p]),
-    "fbbev_voxel_prepare_cams": (
-        ctypes.c_int, [_p] * 8 + [_i32] * 6 + [_p] * 3 + [_p] * 6 +
-        [_p, _sz, _i32, _p, _sz, _p]),
-    "fbbev_voxel_prepare_can_plan": (ctypes.c_int, [_i32, _i64]),
-    "fbbev_voxel_prepare_sparse": (
         ctypes.c_int, [_p, _p, ctypes.c_float] + [_i32] * 5 + [_p] * 3 +
         [_p] * 6 + [_p, _sz, _i32, _p, _sz, _p]),
-    "fbbev_voxel_prepare_cams_sparse": (
+    "fbbev_voxel_prepare_cams": (
         ctypes.c_int, [_p] * 8 + [_i32, _p, ctypes.c_float] + [_i32] * 5 +
         [_p] * 3 + [_p] * 6 + [_p, _sz, _i32, _p, _sz, _p]),
     "fbbev_lift_tail_fwd": (
@@ -180,7 +170,7 @@ _SIGNATURES = {
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 ERR_UNSUPPORTED = -3    # FBBEV_ERR_UNSUPPORTED
 _lib = None
 

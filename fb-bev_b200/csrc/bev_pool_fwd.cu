@@ -278,22 +278,3 @@ FBBEV_API int fbbev_bev_pool_v2_fwd_dense_planned(
                           interval_starts, interval_lengths, n_intervals_max,
                           pp.meta, c, zyx, n_vox, out, st);
 }
-
-FBBEV_API int fbbev_bev_pool_v2_fwd_dense(
-    const float* depth, const float* feat, const int32_t* ranks_depth,
-    const int32_t* ranks_feat, const int32_t* ranks_bev,
-    const int32_t* interval_starts, const int32_t* interval_lengths,
-    int32_t n_intervals_max, const int32_t* n_intervals_dev, int32_t n_points,
-    int32_t c, int32_t batch, int64_t n_voxels_per_sample, float* out,
-    void* workspace, size_t workspace_bytes, fbbev_stream_t stream) {
-  int rc = fbbev_bev_pool_v2_plan(ranks_bev, interval_starts,
-                                  interval_lengths, n_intervals_max,
-                                  n_intervals_dev, n_points, c, batch,
-                                  n_voxels_per_sample, workspace,
-                                  workspace_bytes, stream);
-  if (rc) return rc;
-  return fbbev_bev_pool_v2_fwd_dense_planned(
-      depth, feat, ranks_depth, ranks_feat, ranks_bev, interval_starts,
-      interval_lengths, n_intervals_max, n_points, c, batch,
-      n_voxels_per_sample, out, workspace, workspace_bytes, stream);
-}

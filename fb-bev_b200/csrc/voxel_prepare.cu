@@ -412,19 +412,12 @@ static int voxel_prepare_impl(
   const size_t need =
       prep_layout(n_pts, n_vox, static_cast<char*>(workspace), &w);
   if (workspace_bytes < need) return FBBEV_ERR_WORKSPACE_TOO_SMALL;
-  cudaStream_t st = as_stream(stream);
-
-  cudaError_t e = cudaMemsetAsync(w.hist, 0, (size_t)n_vox * 2 * 4, st);
-  if (e != cudaSuccess) return (int)e;
-  const unsigned pt_grid = (unsigned)ceil_div64(n_pts, kPrepThreads);
-  const int n_scan_blocks = (int)ceil_div64(n_vox, kScanTile);
   PlanOut plan;
   plan.tile_first = nullptr;
   if (pool_plan) {
     const int64_t zyx = (int64_t)g.gx * g.gy * g.gz;
     const int cap = (int)std::min<int64_t>(n_pts, n_vox);
-    if (!fbbev_voxel_prepare_can_plan(pool_c, zyx))
-      return FBBEV_ERR_UNSUPPORTED;
+    if (pool_c <= 0) return FBBEV_ERR_UNSUPPORTED;
     if (pool_plan_bytes < fbbev_bev_pool_v2_dense_workspace_bytes(
                               B, zyx, cap, (int32_t)n_pts, pool_c))
       return FBBEV_ERR_WORKSPACE_TOO_SMALL;
@@ -436,6 +429,12 @@ static int voxel_prepare_impl(
     plan.n_warps_max = pp.n_warps_max;
     plan.zyx = zyx; plan.n_tiles = pp.n_tiles;
   }
+  cudaStream_t st = as_stream(stream);
+
+  cudaError_t e = cudaMemsetAsync(w.hist, 0, (size_t)n_vox * 2 * 4, st);
+  if (e != cudaSuccess) return (int)e;
+  const unsigned pt_grid = (unsigned)ceil_div64(n_pts, kPrepThreads);
+  const int n_scan_blocks = (int)ceil_div64(n_vox, kScanTile);
   count_launch(5);
   if (coor)
     prep_voxelize_kernel<<<pt_grid, kPrepThreads, 0, st>>>(
@@ -456,7 +455,7 @@ static int voxel_prepare_impl(
   return launch_status();
 }
 
-FBBEV_API int fbbev_voxel_prepare_sparse(
+FBBEV_API int fbbev_voxel_prepare(
     const float* coor, const float* depth_prob, float depth_thresh, int32_t B,
     int32_t N, int32_t D, int32_t H, int32_t W, const float* lo_host,
     const float* iv_host, const float* gs_host, int32_t* ranks_bev,
@@ -472,38 +471,7 @@ FBBEV_API int fbbev_voxel_prepare_sparse(
                             pool_plan_bytes, depth_prob, depth_thresh, stream);
 }
 
-FBBEV_API int fbbev_voxel_prepare(
-    const float* coor, int32_t B, int32_t N, int32_t D, int32_t H, int32_t W,
-    const float* lo_host, const float* iv_host, const float* gs_host,
-    int32_t* ranks_bev, int32_t* ranks_depth, int32_t* ranks_feat,
-    int32_t* interval_starts, int32_t* interval_lengths, int32_t* counts,
-    void* workspace, size_t workspace_bytes, int32_t pool_c, void* pool_plan,
-    size_t pool_plan_bytes, fbbev_stream_t stream) {
-  return fbbev_voxel_prepare_sparse(
-      coor, nullptr, 0.f, B, N, D, H, W, lo_host, iv_host, gs_host, ranks_bev,
-      ranks_depth, ranks_feat, interval_starts, interval_lengths, counts,
-      workspace, workspace_bytes, pool_c, pool_plan, pool_plan_bytes, stream);
-}
-
 FBBEV_API int fbbev_voxel_prepare_cams(
-    const float* frustum_u, const float* frustum_v, const float* frustum_d,
-    const float* inv_post_rots, const float* post_trans, const float* cam2ego,
-    const float* trans, const float* bda, int32_t order_flags, int32_t B,
-    int32_t N, int32_t D, int32_t H, int32_t W, const float* lo_host,
-    const float* iv_host,
-    const float* gs_host, int32_t* ranks_bev, int32_t* ranks_depth,
-    int32_t* ranks_feat, int32_t* interval_starts, int32_t* interval_lengths,
-    int32_t* counts, void* workspace, size_t workspace_bytes, int32_t pool_c,
-    void* pool_plan, size_t pool_plan_bytes, fbbev_stream_t stream) {
-  return fbbev_voxel_prepare_cams_sparse(
-      frustum_u, frustum_v, frustum_d, inv_post_rots, post_trans, cam2ego,
-      trans, bda, order_flags, nullptr, 0.f, B, N, D, H, W, lo_host, iv_host,
-      gs_host, ranks_bev, ranks_depth, ranks_feat, interval_starts,
-      interval_lengths, counts, workspace, workspace_bytes, pool_c, pool_plan,
-      pool_plan_bytes, stream);
-}
-
-FBBEV_API int fbbev_voxel_prepare_cams_sparse(
     const float* frustum_u, const float* frustum_v, const float* frustum_d,
     const float* inv_post_rots, const float* post_trans, const float* cam2ego,
     const float* trans, const float* bda, int32_t order_flags,
@@ -528,9 +496,4 @@ FBBEV_API int fbbev_voxel_prepare_cams_sparse(
                             interval_starts, interval_lengths, counts,
                             workspace, workspace_bytes, pool_c, pool_plan,
                             pool_plan_bytes, depth_prob, depth_thresh, stream);
-}
-
-// every dense-pooling workspace holds the plan tables, whatever the shape
-FBBEV_API int fbbev_voxel_prepare_can_plan(int32_t pool_c, int64_t zyx) {
-  return pool_c > 0 && zyx > 0 ? 1 : 0;
 }

@@ -7,11 +7,11 @@ meaning, output layout):
   reference-layout kernels; ``forward`` returns ``(B, Z, Y, X, C)``.
 * ``bev_pool_v2()``     -- bev_pool.py:84-90: returns the contiguous
   ``(B, C, Z, Y, X)`` tensor.  Here it is the library's dense op
-  (``fbbev_bev_pool_v2_fwd_dense[_planned]``), which writes the volume in that
-  layout directly instead of memset + kernel + transpose copy: two kernels
-  that write every element once on the shapes the model runs, and zero fill +
-  the interval kernel with the transpose folded into its stores on any other
-  shape.
+  (``fbbev_bev_pool_v2_plan`` + ``_fwd_dense_planned``), which writes the
+  volume in that layout directly instead of memset + kernel + transpose copy:
+  two kernels that write every element once on the shapes the model runs, and
+  zero fill + the interval kernel with the transpose folded into its stores on
+  any other shape.
 * ``voxel_pooling_prepare_v2`` -- device implementation of
   view_transformer.py:547-605 (``fbbev_voxel_prepare``).
 
@@ -99,6 +99,17 @@ class QuickCumsumCuda(torch.autograd.Function):
 KERNEL_HOOK = None
 
 
+def _dense_workspace(L, B, zyx, n_int, n_points, C):
+    """``(cap, nbytes)``: the interval capacity of a dense-pooling workspace
+    for an index of ``n_int`` interval slots, and its size in bytes.  An index
+    can never hold more intervals than there are voxels: the cap bounds the
+    V[n_intervals][C] workspace of the sync-free path (whose index buffers are
+    n_points long) -- 1.7 GB -> 0.8 GB for 16 frames of 200x200x16."""
+    cap = min(n_int, B * zyx)
+    return cap, L.fbbev_bev_pool_v2_dense_workspace_bytes(B, zyx, cap,
+                                                          n_points, C)
+
+
 def _planned_workspace(L, dev, shape, ranks_bev, interval_starts,
                        interval_lengths, n_intervals_dev, plan):
     """``(ws, ws_bytes, n_int_cap)``: a dense-pooling workspace holding the
@@ -108,16 +119,12 @@ def _planned_workspace(L, dev, shape, ranks_bev, interval_starts,
     enqueued on the current stream of ``dev``)."""
     B, Z, Y, X, C = shape
     n_points = ranks_bev.shape[0]
-    # an index can never hold more intervals than there are voxels: bounds the
-    # V[n_intervals][C] workspace of the sync-free path (whose index buffers
-    # are n_points long) -- 1.7 GB -> 0.8 GB for 16 frames of 200x200x16
-    cap = min(interval_lengths.shape[0], B * Z * Y * X)
+    cap, ws_bytes = _dense_workspace(L, B, Z * Y * X, interval_lengths.shape[0],
+                                     n_points, C)
     if plan is not None:
-        ws, ws_bytes, pshape, pcap = plan
+        pws, pbytes, pshape, pcap = plan
         if tuple(pshape) == shape and pcap == cap:
-            return ws, ws_bytes, cap
-    ws_bytes = L.fbbev_bev_pool_v2_dense_workspace_bytes(B, Z * Y * X, cap,
-                                                         n_points, C)
+            return pws, pbytes, cap
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
         rc = L.fbbev_bev_pool_v2_plan(
@@ -594,10 +601,8 @@ def _plan_workspace(L, dev, B, gs, n_pts, pool_channels):
     if not pool_channels:
         return None, 0, None
     X, Y, Z = int(gs[0]), int(gs[1]), int(gs[2])
-    zyx = Z * Y * X
     C = int(pool_channels)
-    cap = min(n_pts, B * zyx)
-    nbytes = L.fbbev_bev_pool_v2_dense_workspace_bytes(B, zyx, cap, n_pts, C)
+    cap, nbytes = _dense_workspace(L, B, Z * Y * X, n_pts, n_pts, C)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     return ws, nbytes, (ws, nbytes, (B, Z, Y, X, C), cap)
 
@@ -610,6 +615,33 @@ def _depth_arg(depth, n_pts, dev):
     d = depth.detach().contiguous().float()
     assert d.numel() == n_pts and d.device == dev
     return d
+
+
+def _prepare(entry, geometry, dev, B, N, D, H, W, grid_lower_bound,
+             grid_interval, grid_size, pool_channels, depth, depth_thresh):
+    """Build a :class:`VoxelIndex` with the C entry point named ``entry``,
+    called with its ``geometry`` arguments followed by the depth threshold,
+    sizes, grid, index buffers, workspace and pooling plan laid out here."""
+    lo, iv, gs = ([float(v) for v in torch.as_tensor(t).float().cpu()]
+                  for t in (grid_lower_bound, grid_interval, grid_size))
+    n_pts = B * N * D * H * W
+    n_vox = B * int(gs[0]) * int(gs[1]) * int(gs[2])
+    L = _lib.lib()
+    idx = torch.empty((5, n_pts), dtype=torch.int32, device=dev)
+    counts = torch.empty(2, dtype=torch.int32, device=dev)
+    ws_bytes = L.fbbev_voxel_prepare_workspace_bytes(n_pts, n_vox)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    pws, pbytes, plan = _plan_workspace(L, dev, B, gs, n_pts, pool_channels)
+    dprob = _depth_arg(depth, n_pts, dev)
+    with torch.cuda.device(dev):
+        rc = getattr(L, entry)(
+            *geometry, _lib.ptr(dprob), float(depth_thresh), B, N, D, H, W,
+            _lib.c_floats(lo), _lib.c_floats(iv), _lib.c_floats(gs),
+            *(_lib.ptr(t) for t in idx), _lib.ptr(counts), _lib.ptr(ws),
+            ws_bytes, int(pool_channels or 0), _lib.ptr(pws), pbytes,
+            _lib.stream_ptr(dev))
+    _lib.check(rc, entry)
+    return VoxelIndex(*idx, counts, plan)
 
 
 def voxel_pooling_prepare_v2(coor, grid_lower_bound, grid_interval, grid_size,
@@ -630,28 +662,9 @@ def voxel_pooling_prepare_v2(coor, grid_lower_bound, grid_interval, grid_size,
     coor = coor.contiguous().float()
     B, N, D, H, W, three = coor.shape
     assert three == 3
-    lo = [float(v) for v in torch.as_tensor(grid_lower_bound).float().cpu()]
-    iv = [float(v) for v in torch.as_tensor(grid_interval).float().cpu()]
-    gs = [float(v) for v in torch.as_tensor(grid_size).float().cpu()]
-    n_pts = B * N * D * H * W
-    n_vox = B * int(gs[0]) * int(gs[1]) * int(gs[2])
-    L = _lib.lib()
-    idx = torch.empty((5, n_pts), dtype=torch.int32, device=dev)
-    counts = torch.empty(2, dtype=torch.int32, device=dev)
-    ws_bytes = L.fbbev_voxel_prepare_workspace_bytes(n_pts, n_vox)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    pws, pbytes, plan = _plan_workspace(L, dev, B, gs, n_pts, pool_channels)
-    dprob = _depth_arg(depth, n_pts, dev)
-    with torch.cuda.device(dev):
-        rc = L.fbbev_voxel_prepare_sparse(
-            _lib.ptr(coor), _lib.ptr(dprob), float(depth_thresh), B, N, D, H,
-            W, _lib.c_floats(lo), _lib.c_floats(iv),
-            _lib.c_floats(gs), _lib.ptr(idx[0]), _lib.ptr(idx[1]),
-            _lib.ptr(idx[2]), _lib.ptr(idx[3]), _lib.ptr(idx[4]),
-            _lib.ptr(counts), _lib.ptr(ws), ws_bytes, int(pool_channels or 0),
-            _lib.ptr(pws), pbytes, _lib.stream_ptr(dev))
-    _lib.check(rc, 'fbbev_voxel_prepare')
-    return VoxelIndex(idx[0], idx[1], idx[2], idx[3], idx[4], counts, plan)
+    return _prepare('fbbev_voxel_prepare', (_lib.ptr(coor),), dev, B, N, D, H,
+                    W, grid_lower_bound, grid_interval, grid_size,
+                    pool_channels, depth, depth_thresh)
 
 
 def voxel_pooling_prepare_from_cams(frustum_axes, inv_post_rots, post_trans,
@@ -677,28 +690,7 @@ def voxel_pooling_prepare_from_cams(frustum_axes, inv_post_rots, post_trans,
     B, N = mats[0].shape[:2]
     D, H, W = fd.shape[0], fv.shape[0], fu.shape[0]
     assert D == depth_bins
-    lo = [float(v) for v in torch.as_tensor(grid_lower_bound).float().cpu()]
-    iv = [float(v) for v in torch.as_tensor(grid_interval).float().cpu()]
-    gs = [float(v) for v in torch.as_tensor(grid_size).float().cpu()]
-    n_pts = B * N * D * H * W
-    n_vox = B * int(gs[0]) * int(gs[1]) * int(gs[2])
-    L = _lib.lib()
-    idx = torch.empty((5, n_pts), dtype=torch.int32, device=dev)
-    counts = torch.empty(2, dtype=torch.int32, device=dev)
-    ws_bytes = L.fbbev_voxel_prepare_workspace_bytes(n_pts, n_vox)
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    pws, pbytes, plan = _plan_workspace(L, dev, B, gs, n_pts, pool_channels)
-    dprob = _depth_arg(depth, n_pts, dev)
-    with torch.cuda.device(dev):
-        rc = L.fbbev_voxel_prepare_cams_sparse(
-            _lib.ptr(fu), _lib.ptr(fv), _lib.ptr(fd), _lib.ptr(mats[0]),
-            _lib.ptr(mats[1]), _lib.ptr(mats[2]), _lib.ptr(mats[3]),
-            _lib.ptr(mats[4]), order, _lib.ptr(dprob), float(depth_thresh), B,
-            N, D, H, W, _lib.c_floats(lo),
-            _lib.c_floats(iv), _lib.c_floats(gs), _lib.ptr(idx[0]),
-            _lib.ptr(idx[1]), _lib.ptr(idx[2]), _lib.ptr(idx[3]),
-            _lib.ptr(idx[4]), _lib.ptr(counts), _lib.ptr(ws), ws_bytes,
-            int(pool_channels or 0), _lib.ptr(pws), pbytes,
-            _lib.stream_ptr(dev))
-    _lib.check(rc, 'fbbev_voxel_prepare_cams')
-    return VoxelIndex(idx[0], idx[1], idx[2], idx[3], idx[4], counts, plan)
+    geometry = [_lib.ptr(t) for t in (fu, fv, fd, *mats)] + [order]
+    return _prepare('fbbev_voxel_prepare_cams', geometry, dev, B, N, D, H, W,
+                    grid_lower_bound, grid_interval, grid_size, pool_channels,
+                    depth, depth_thresh)

@@ -18,7 +18,7 @@ mlp_input)]``), return value ``(bev_feat, depth)`` and state-dict keys
 What runs underneath: the tail of ``forward`` -- channel split, softmax over
 the depth bins, and the NCHW -> NHWC copy the pooling op would start with --
 is one launch (``ops.lift_tail``); index building with the threshold is the
-device counting sort (``fbbev_voxel_prepare(_cams)_sparse``); pooling is the
+device counting sort (``fbbev_voxel_prepare(_cams)``); pooling is the
 dense op.  The ``depth_net`` convolution stays a library call (cuDNN): it is
 the step before the path.
 """
@@ -26,11 +26,10 @@ import torch
 import torch.nn as nn
 
 from ..ops import depth_loss as _depth_loss
-from ..ops.bev_pool_v2 import (voxel_pooling_prepare_from_cams,
-                               voxel_pooling_prepare_v2)
+from ..ops.bev_pool_v2 import voxel_pooling_prepare_v2
 from ..ops.lift_tail import lift_tail
 from ..registry import register
-from .forward_projection import _LSSBase, inv3x3_many
+from .forward_projection import _LSSBase
 
 __all__ = ['LSSViewTransformer', 'LSSViewTransformer2',
            'LSSViewTransformerBEVDepth', 'DEPTH_THRESHOLD']
@@ -50,8 +49,6 @@ class LSSViewTransformer(_LSSBase):
         uniform (bool): uniform depth distribution (``depth_digit * 0``, :316).
     """
 
-    depth_threshold = None      # LSSViewTransformer2 sets 0.01
-
     def __init__(self, grid_config, input_size, downsample=16, in_channels=512,
                  out_channels=64, accelerate=False, uniform=False,
                  with_cp=False):
@@ -63,26 +60,6 @@ class LSSViewTransformer(_LSSBase):
         self.in_channels = in_channels
         self.depth_net = nn.Conv2d(in_channels, self.D + self.out_channels,
                                    kernel_size=1, padding=0)
-
-    # -- index ------------------------------------------------------------
-    def _build_index(self, cam_params, depth, pool_channels=None):
-        """VoxelIndex of this call: geometry (fused or ``get_lidar_coor``),
-        bounds test and -- LSSViewTransformer2 -- the depth threshold."""
-        thr = self.depth_threshold
-        kw = dict(pool_channels=pool_channels)
-        if thr is not None:
-            kw.update(depth=depth, depth_thresh=thr)
-        if self.fused_geometry:
-            rots, trans, intrins, post_rots, post_trans, bda = cam_params
-            inv_pr, inv_k = inv3x3_many(post_rots, intrins)
-            return voxel_pooling_prepare_from_cams(
-                self._frustum_axes(rots.device), inv_pr, post_trans,
-                rots.matmul(inv_k), trans, bda, self.D, self.grid_lower_bound,
-                self.grid_interval, self.grid_size, **kw)
-        coor = self.get_lidar_coor(*cam_params)
-        return voxel_pooling_prepare_v2(coor, self.grid_lower_bound,
-                                        self.grid_interval, self.grid_size,
-                                        **kw)
 
     @staticmethod
     def _collapse(bev_feat):
@@ -99,13 +76,9 @@ class LSSViewTransformer(_LSSBase):
         if self.initial_flag:
             # static rig: remember the cameras the index belongs to; the
             # reference-visible attributes are filled from the geometric index
+            # (no depth: no threshold)
             self._cached_cams = [t.detach().clone() for t in input[1:7]]
-            thr, self.depth_threshold = self.depth_threshold, None
-            try:
-                self.init_acceleration_v2(
-                    self._build_index(self._cached_cams, None))
-            finally:
-                self.depth_threshold = thr
+            self.init_acceleration_v2(self._build_index(self._cached_cams))
             self.initial_flag = False
 
     # -- necks/view_transformer.py:266-289 ---------------------------------

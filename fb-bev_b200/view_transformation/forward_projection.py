@@ -11,7 +11,7 @@ What changed underneath:
 * ``voxel_pooling_prepare_v2`` (view_transformer.py:547-605) runs as six small
   CUDA kernels with no host synchronisation (``fbbev_voxel_prepare``);
 * ``bev_pool_v2`` (bev_pool.py:84-90) is one fused kernel that writes the
-  ``(B,C,Z,Y,X)`` volume once (``fbbev_bev_pool_v2_fwd_dense``);
+  ``(B,C,Z,Y,X)`` volume once (``fbbev_bev_pool_v2_fwd_dense_planned``);
 * ``accelerate=True`` caches the device index (the reference's 3-D class
   asserts out at view_transformer.py:628; the 2-D class supports it, :271-283).
 
@@ -80,6 +80,8 @@ class _LSSBase(BaseModule):
     """
 
     fused_geometry = True
+    # LSSViewTransformer2 keeps the points whose depth probability exceeds it
+    depth_threshold = None
 
     def __init__(self, grid_config, input_size, downsample, accelerate,
                  uniform, with_cp):
@@ -156,27 +158,41 @@ class _LSSBase(BaseModule):
         return cache[key]
 
     def prepare_index_from_cams(self, rots, trans, cam2imgs, post_rots,
-                                post_trans, bda, pool_channels=None):
+                                post_trans, bda, pool_channels=None, **thresh):
         """Index straight from the camera parameters (fused geometry).  The
         two 3x3 products the reference forms before touching the points
         (view_transformer.py:483-491) are formed here by the same torch ops
         (inv_ex == torch.inverse without the host-side error check; the two
-        inverses share one batched call)."""
+        inverses share one batched call).  ``thresh``: ``depth`` and
+        ``depth_thresh`` of :func:`voxel_pooling_prepare_from_cams`."""
         inv_pr, inv_k = inv3x3_many(post_rots, cam2imgs)
         cam2ego = rots.matmul(inv_k)
         return voxel_pooling_prepare_from_cams(
             self._frustum_axes(rots.device), inv_pr, post_trans, cam2ego,
             trans, bda, self.D, self.grid_lower_bound, self.grid_interval,
-            self.grid_size, pool_channels=pool_channels)
+            self.grid_size, pool_channels=pool_channels, **thresh)
 
     # -- view_transformer.py:547-605 ------------------------------------
-    def prepare_index(self, coor, pool_channels=None):
+    def prepare_index(self, coor, pool_channels=None, **thresh):
         """Device-resident index of ``coor`` (no host sync).  ``pool_channels``:
         the channel count of the pooling call that follows, so that the index
-        builder can fill that call's plan while it scans."""
+        builder can fill that call's plan while it scans.  ``thresh``:
+        ``depth`` and ``depth_thresh`` of :func:`voxel_pooling_prepare_v2`."""
         return voxel_pooling_prepare_v2(coor, self.grid_lower_bound,
                                         self.grid_interval, self.grid_size,
-                                        pool_channels=pool_channels)
+                                        pool_channels=pool_channels, **thresh)
+
+    def _build_index(self, cam_params, depth=None, pool_channels=None):
+        """VoxelIndex of this call's cameras: geometry fused into the index
+        builder or through ``get_lidar_coor`` (``fused_geometry``), bounds
+        test and -- with a ``depth_threshold`` and ``depth`` (B,N,D,H,W) --
+        the depth threshold."""
+        kw = dict(pool_channels=pool_channels)
+        if self.depth_threshold is not None and depth is not None:
+            kw.update(depth=depth, depth_thresh=self.depth_threshold)
+        if self.fused_geometry:
+            return self.prepare_index_from_cams(*cam_params, **kw)
+        return self.prepare_index(self.get_lidar_coor(*cam_params), **kw)
 
     def voxel_pooling_prepare_v2(self, coor):
         """Same return contract as the reference: five exact-length int32
@@ -196,11 +212,7 @@ class _LSSBase(BaseModule):
 
     def pre_compute(self, cam_params):
         if self.initial_flag:
-            if self.fused_geometry:
-                self.init_acceleration_v2(
-                    self.prepare_index_from_cams(*cam_params))
-            else:
-                self.init_acceleration_v2(self.get_lidar_coor(*cam_params))
+            self.init_acceleration_v2(self._build_index(cam_params))
             self.initial_flag = False
 
     def _bev_feat_shape(self, depth, feat_nhwc):
@@ -269,12 +281,7 @@ class LSSViewTransformerFunction3D(_LSSBase):
             bev_feat = self._pool(self._index, depth, tran_feat, nhwc)
             return bev_feat.permute(0, 1, 3, 4, 2)
         C = tran_feat.shape[-1 if nhwc else 2]
-        if self.fused_geometry:
-            idx = self.prepare_index_from_cams(*cam_params, pool_channels=C)
-            return self._pool(idx, depth, tran_feat, nhwc).permute(
-                0, 1, 3, 4, 2)
-        coor = self.get_lidar_coor(*cam_params)
-        idx = self.prepare_index(coor, pool_channels=C)
+        idx = self._build_index(cam_params, pool_channels=C)
         return self._pool(idx, depth, tran_feat, nhwc).permute(0, 1, 3, 4, 2)
 
     def view_transform(self, cam_params, depth, tran_feat, nhwc=False):
@@ -299,12 +306,8 @@ class LSSViewTransformerFunction3D(_LSSBase):
         if self.accelerate:
             self.pre_compute(cam_params)
             idx = self._index
-        elif self.fused_geometry:
-            idx = self.prepare_index_from_cams(*cam_params,
-                                               pool_channels=shape[-1])
         else:
-            idx = self.prepare_index(self.get_lidar_coor(*cam_params),
-                                     pool_channels=shape[-1])
+            idx = self._build_index(cam_params, pool_channels=shape[-1])
         if torch.is_grad_enabled() and (context.requires_grad or
                                         depth.requires_grad):
             return DeferredVolumeTrain(depth, feat, idx, shape)
@@ -353,11 +356,8 @@ class LSSViewTransformerFunction(_LSSBase):
         if self.accelerate:
             # the reference squeezes Z here (:283): 4-D only when Z == 1
             return self._pool(self._index, depth, tran_feat).squeeze(2)
-        if self.fused_geometry:
-            idx = self.prepare_index_from_cams(*cam_params)
-            return self._collapse(self._pool(idx, depth, tran_feat))
-        coor = self.get_lidar_coor(*cam_params)
-        return self.voxel_pooling_v2(coor, depth, tran_feat)
+        return self._collapse(self._pool(self._build_index(cam_params), depth,
+                                         tran_feat))
 
     def view_transform(self, cam_params, depth, tran_feat):
         if self.accelerate:

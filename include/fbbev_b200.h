@@ -31,7 +31,7 @@ extern "C" {
 #define FBBEV_ERR_WORKSPACE_TOO_SMALL (-2)
 #define FBBEV_ERR_UNSUPPORTED (-3)
 
-#define FBBEV_ABI_VERSION 4
+#define FBBEV_ABI_VERSION 5
 
 typedef void* fbbev_stream_t; /* cudaStream_t */
 
@@ -75,13 +75,22 @@ int fbbev_bev_pool_v2_fwd(const float* depth, const float* feat,
  * of their voxel rank ranks_bev[interval_starts[i]], one interval per voxel.
  * Out-of-range ranks are ignored (memory-safe).
  *
+ * Two calls:
+ *   _plan     builds the tile table of a given (index, C) into `workspace`
+ *             (>= fbbev_bev_pool_v2_dense_workspace_bytes(...) bytes);
+ *   _planned  runs the pooling kernels from it.  The workspace doubles as
+ *             their scratch, so `_planned` writes it as well: one workspace
+ *             per concurrent stream.
+ * A caller that reuses an index (static camera rig, `accelerate=True`,
+ * view_transformer.py:261-283) plans once; fbbev_voxel_prepare(_cams) can
+ * fill the plan while it builds the index, so no `_plan` launch is needed.
+ *
  * n_intervals_dev: optional device int32 holding the live interval count
  *   (<= n_intervals_max); NULL means n_intervals_max is the count.  This lets
  *   the prepare -> pool chain run without a host sync / under CUDA graphs.
  * n_points = number of entries in ranks_bev / ranks_depth / ranks_feat (an
  *   upper bound of the kept points when the buffers are over-allocated).
  * n_voxels_per_sample = Z*Y*X.
- * workspace: >= fbbev_bev_pool_v2_dense_workspace_bytes(...) bytes.
  * Any C > 0 and volume.  Two kernels write every element once when
  * C % 4 == 0, Z*Y*X % 4 == 0, 4 <= C <= 512 and B*Z*Y*X < 2^31 (every shape
  * the model runs; out must then be 16-byte aligned); any other shape is
@@ -93,21 +102,6 @@ size_t fbbev_bev_pool_v2_dense_workspace_bytes(int32_t batch,
                                                int64_t n_voxels_per_sample,
                                                int32_t n_intervals_max,
                                                int32_t n_points, int32_t c);
-int fbbev_bev_pool_v2_fwd_dense(
-    const float* depth, const float* feat, const int32_t* ranks_depth,
-    const int32_t* ranks_feat, const int32_t* ranks_bev,
-    const int32_t* interval_starts, const int32_t* interval_lengths,
-    int32_t n_intervals_max, const int32_t* n_intervals_dev, int32_t n_points,
-    int32_t c, int32_t batch, int64_t n_voxels_per_sample, float* out,
-    void* workspace, size_t workspace_bytes, fbbev_stream_t stream);
-
-/*
- * The two halves of fbbev_bev_pool_v2_fwd_dense, for callers that reuse an
- * index (static camera rig, `accelerate=True`, view_transformer.py:261-283):
- * `plan` builds the tile table for a given (index, C) once; `_planned` then
- * runs only the pooling kernels (the workspace doubles as their scratch, so it
- * is written by `_planned` as well; one workspace per concurrent stream).
- */
 int fbbev_bev_pool_v2_plan(const int32_t* ranks_bev,
                            const int32_t* interval_starts,
                            const int32_t* interval_lengths,
@@ -273,21 +267,39 @@ int fbbev_bev_pool_v2_bwd_ordered(
  * Voxel rank is computed in exact integer arithmetic; the reference computes
  * it in float32 (:586-589), which is identical while B*Z*Y*X < 2^24.
  * Requires B*Z*Y*X < 2^31 and B*N*D*H*W < 2^31.
+ *
+ * depth_prob (may be NULL: no threshold) adds the depth-threshold
+ * sparsification of the BEVDet-lineage transformer
+ *   mmdet3d/models/necks/view_transformer.py:520-578 (LSSViewTransformer2.
+ *   voxel_pooling_prepare_v2: `kept = kept & (depth.view(-1) > 0.01)`, :556-557)
+ *   and its cached-index form (:645-678: the geometric index filtered by
+ *   `(depth.view(-1) > 0.01)[self.kept]` on every forward):
+ * depth_prob (B,N,D,H,W) fp32 -- the tensor the pooling op will read, indexed
+ * by the point index (ranks_depth == arange); a point is kept when
+ * depth_prob[p] > depth_thresh (strict, as the reference).
+ *
+ * pool_plan (may be NULL): a dense-pooling workspace of
+ * fbbev_bev_pool_v2_dense_workspace_bytes(B, Z*Y*X, min(n_points, B*Z*Y*X),
+ * n_points, pool_c) bytes.  When given, the scan over the voxel histogram also
+ * fills the pooling plan (what fbbev_bev_pool_v2_plan computes in a launch of
+ * its own), so the index can go straight to fbbev_bev_pool_v2_fwd_dense_planned
+ * / _sums_planned with the same workspace and n_intervals_max = min(n_points,
+ * B*Z*Y*X).  A plan needs pool_c > 0, else FBBEV_ERR_UNSUPPORTED.
+ * Argument errors are reported before anything is enqueued.
  */
 size_t fbbev_voxel_prepare_workspace_bytes(int64_t n_points,
                                            int64_t n_voxels_total);
-int fbbev_voxel_prepare(const float* coor, int32_t B, int32_t N, int32_t D,
-                        int32_t H, int32_t W, const float* lo_host,
-                        const float* iv_host, const float* gs_host,
-                        int32_t* ranks_bev, int32_t* ranks_depth,
-                        int32_t* ranks_feat, int32_t* interval_starts,
-                        int32_t* interval_lengths, int32_t* counts,
-                        void* workspace, size_t workspace_bytes, int32_t pool_c,
-                        void* pool_plan, size_t pool_plan_bytes,
-                        fbbev_stream_t stream);
+int fbbev_voxel_prepare(
+    const float* coor, const float* depth_prob, float depth_thresh, int32_t B,
+    int32_t N, int32_t D, int32_t H, int32_t W, const float* lo_host,
+    const float* iv_host, const float* gs_host, int32_t* ranks_bev,
+    int32_t* ranks_depth, int32_t* ranks_feat, int32_t* interval_starts,
+    int32_t* interval_lengths, int32_t* counts, void* workspace,
+    size_t workspace_bytes, int32_t pool_c, void* pool_plan,
+    size_t pool_plan_bytes, fbbev_stream_t stream);
 
 /*
- * voxel_pooling_prepare_v2 with get_lidar_coor fused in
+ * fbbev_voxel_prepare with get_lidar_coor fused in
  *   (view_transformer.py:458-498 + 547-605): the (B,N,D,H,W,3) coordinate tensor
  *   is never materialised.  frustum_u [W], frustum_v [H], frustum_d [D] are the
  *   three axes of the frustum template (create_frustum, :389-411);
@@ -301,17 +313,8 @@ int fbbev_voxel_prepare(const float* coor, int32_t B, int32_t N, int32_t D,
  * column-major matrix (the layout torch.inverse returns) is broadcast over the
  * whole batch.  order_flags: bit 0 inv_post_rots, bit 1 cam2ego, bit 2 bda.
  * The index is bit-identical to fbbev_voxel_prepare on get_lidar_coor's output.
- *
- * pool_plan (both prepare entry points; may be NULL): a dense-pooling workspace
- * of fbbev_bev_pool_v2_dense_workspace_bytes(B, Z*Y*X, min(n_points, B*Z*Y*X),
- * n_points, pool_c) bytes.  When given, the scan over the voxel histogram also
- * fills the pooling plan (what fbbev_bev_pool_v2_plan computes in a launch of
- * its own), so the index can go straight to fbbev_bev_pool_v2_fwd_dense_planned
- * / _sums_planned with the same workspace and n_intervals_max = min(n_points,
- * B*Z*Y*X).  Needs fbbev_voxel_prepare_can_plan(pool_c, Z*Y*X) != 0, else
- * FBBEV_ERR_UNSUPPORTED; it is 1 for every pool_c > 0 and Z*Y*X > 0.
+ * Everything else (depth_prob, pool_plan) as fbbev_voxel_prepare.
  */
-int fbbev_voxel_prepare_can_plan(int32_t pool_c, int64_t n_voxels_per_sample);
 #define FBBEV_ORDER_SEQ_A 1
 #define FBBEV_ORDER_SEQ_B 2
 #define FBBEV_ORDER_SEQ_C 4
@@ -324,37 +327,6 @@ int fbbev_voxel_prepare_can_plan(int32_t pool_c, int64_t n_voxels_per_sample);
  * _lib.matmul_order_codes). */
 #define FBBEV_ORDER_EXPLICIT 8
 int fbbev_voxel_prepare_cams(
-    const float* frustum_u, const float* frustum_v, const float* frustum_d,
-    const float* inv_post_rots, const float* post_trans, const float* cam2ego,
-    const float* trans, const float* bda, int32_t order_flags, int32_t B,
-    int32_t N, int32_t D, int32_t H, int32_t W, const float* lo_host,
-    const float* iv_host, const float* gs_host, int32_t* ranks_bev,
-    int32_t* ranks_depth, int32_t* ranks_feat, int32_t* interval_starts,
-    int32_t* interval_lengths, int32_t* counts, void* workspace,
-    size_t workspace_bytes, int32_t pool_c, void* pool_plan,
-    size_t pool_plan_bytes, fbbev_stream_t stream);
-
-/*
- * The same two index builders with the depth-threshold sparsification of the
- * BEVDet-lineage transformer
- *   mmdet3d/models/necks/view_transformer.py:520-578 (LSSViewTransformer2.
- *   voxel_pooling_prepare_v2: `kept = kept & (depth.view(-1) > 0.01)`, :556-557)
- *   and its cached-index form (:645-678: the geometric index filtered by
- *   `(depth.view(-1) > 0.01)[self.kept]` on every forward).
- * depth_prob (B,N,D,H,W) fp32 -- the tensor the pooling op will read, indexed
- * by the point index (ranks_depth == arange) -- may be NULL (no threshold);
- * a point is kept when depth_prob[p] > depth_thresh (strict, as the reference).
- * Everything else as fbbev_voxel_prepare / fbbev_voxel_prepare_cams.
- */
-int fbbev_voxel_prepare_sparse(
-    const float* coor, const float* depth_prob, float depth_thresh, int32_t B,
-    int32_t N, int32_t D, int32_t H, int32_t W, const float* lo_host,
-    const float* iv_host, const float* gs_host, int32_t* ranks_bev,
-    int32_t* ranks_depth, int32_t* ranks_feat, int32_t* interval_starts,
-    int32_t* interval_lengths, int32_t* counts, void* workspace,
-    size_t workspace_bytes, int32_t pool_c, void* pool_plan,
-    size_t pool_plan_bytes, fbbev_stream_t stream);
-int fbbev_voxel_prepare_cams_sparse(
     const float* frustum_u, const float* frustum_v, const float* frustum_d,
     const float* inv_post_rots, const float* post_trans, const float* cam2ego,
     const float* trans, const float* bda, int32_t order_flags,

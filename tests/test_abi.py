@@ -30,7 +30,7 @@ def test_header_symbols_all_exported():
 def test_abi_version_and_error_strings():
     from fbbev_b200 import _lib
     L = _lib.lib()
-    assert L.fbbev_abi_version() == 4
+    assert L.fbbev_abi_version() == 5
     assert L.fbbev_error_string(0) == b"ok"
     assert b"workspace" in L.fbbev_error_string(-2)
     assert L.fbbev_bev_pool_v2_dense_workspace_bytes(1, 640000, 1000, 2000, 80) >= 4 * (
@@ -44,8 +44,6 @@ def test_dense_pool_plan_covers_every_shape():
     path (C <= 512), so a C = 1024 workspace holds the plan tables alone."""
     from fbbev_b200 import _lib
     L = _lib.lib()
-    assert L.fbbev_voxel_prepare_can_plan(13, 105) == 1
-    assert L.fbbev_voxel_prepare_can_plan(1024, 64) == 1
     ws = L.fbbev_bev_pool_v2_dense_workspace_bytes
     n_int, n_pts = 1000, 2000
     assert ws(1, 64, n_int, n_pts, 512) >= n_int * 512 * 4
@@ -78,6 +76,13 @@ def test_argument_validation_without_gpu():
     assert L.fbbev_da_sca_fwd(*([None] * 10), 1, 6, 10, 10, 8, 10, 1, 7, 4,
                               80, None, None, 0, 0, None) == -1  # points % Z != 0
     assert L.fbbev_da_sca_workspace_bytes(2, 6) >= 2 * 6 * 4
+    # the index builder refuses a pooling plan without channels
+    fake = 1 << 20          # a non-NULL pointer that is never dereferenced
+    grid = [_lib.c_floats(v) for v in ([0, 0, 0], [1, 1, 1], [4, 4, 4])]
+    need = L.fbbev_voxel_prepare_workspace_bytes(16, 64)
+    assert L.fbbev_voxel_prepare(fake, None, 0.0, 1, 1, 1, 4, 4, *grid,
+                                 *([fake] * 6), fake, need, 0, fake, 1 << 20,
+                                 None) == -3
 
 
 def test_no_cpu_fallback():

@@ -202,7 +202,7 @@ def test_adjoint_deterministic_and_batch_independent():
     for b in (0, 2):
         err = float((outs[0][b].double() - want[b]).abs().max())
         assert err <= 1e-5 * max(1.0, float(want[b].abs().max())), err
-    assert _lib.lib().fbbev_abi_version() == 4
+    assert _lib.lib().fbbev_abi_version() == 5
 
 
 # -- the module -----------------------------------------------------------------

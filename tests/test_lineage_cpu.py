@@ -87,7 +87,7 @@ def test_header_declares_the_new_entry_points():
     here = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     hdr = open(os.path.join(here, "include", "fbbev_b200.h")).read()
     for sym in ("fbbev_ffn_fwd", "fbbev_ffn_supported", "fbbev_lift_tail_fwd",
-                "fbbev_voxel_prepare_sparse", "fbbev_voxel_prepare_cams_sparse",
+                "fbbev_voxel_prepare", "fbbev_voxel_prepare_cams",
                 "fbbev_bev_mask_fold", "fbbev_bev_mask_fold_workspace_bytes"):
         assert sym + "(" in hdr, sym
         assert hasattr(__import__("fbbev_b200")._lib.lib(), sym)

@@ -9,6 +9,7 @@ sits on every pixel, so every case has queries on the four borders and
 corners, where the window is shifted inwards and corners off the map read as
 zeros."""
 import math
+import os
 
 import pytest
 import torch
@@ -84,22 +85,42 @@ def _both(args, W):
     return tiled
 
 
+_DISPATCH_NAMES = r"""
+import json, sys
+sys.path[:0] = sys.argv[1:3]
+from fbbev_b200.ops.ms_deform_attn import ms_deform_attn_fused
+from test_msda_self_smem_gpu import _inputs, _kernels
+print(json.dumps([sorted(_kernels(
+    lambda: ms_deform_attn_fused(*_inputs(H, W, ch=ch), pw)))
+    for H, W, ch, pw in json.loads(sys.argv[3])]))
+"""
+
+
 def test_dispatch_reaches_the_tile_kernel():
     """8 x 10 self-attention on a map of one window or more runs the tile
-    kernel; a smaller map, another head width or patch_w = 0 do not."""
-    from fbbev_b200.ops.ms_deform_attn import ms_deform_attn_fused
+    kernel; a smaller map, another head width or patch_w = 0 do not.  The
+    profiler names the kernels in a process of its own: in a process that has
+    run many other tests, it can stop reporting kernel records at all."""
+    import json
+    import subprocess
+    import sys
 
-    def ran(args, W):
-        names = _kernels(lambda: ms_deform_attn_fused(*args, W))
-        if not any("fbbev::" in n for n in names):
-            pytest.skip("the profiler reported no library kernel")
-        return any(KERNEL in n for n in names)
-    assert ran(_inputs(WINDOW, 40), 40)
-    assert ran(_inputs(200, 200), 200)
-    assert not ran(_inputs(WINDOW - 1, 40), 40)
-    assert not ran(_inputs(40, WINDOW - 1), WINDOW - 1)
-    assert not ran(_inputs(40, 40), 0)
-    assert not ran(_inputs(40, 40, ch=32), 40)
+    from conftest import ROOT
+    cases = [(WINDOW, 40, CH, 40), (200, 200, CH, 200),
+             (WINDOW - 1, 40, CH, 40), (40, WINDOW - 1, CH, WINDOW - 1),
+             (40, 40, CH, 0), (40, 40, 32, 40)]
+    flags = ["-I"] if sys.flags.isolated else \
+        ["-s"] if sys.flags.no_user_site else []
+    res = subprocess.run(
+        [sys.executable, *flags, "-c", _DISPATCH_NAMES, ROOT,
+         os.path.dirname(os.path.abspath(__file__)), json.dumps(cases)],
+        stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True)
+    assert res.returncode == 0, res.stderr[-2000:]
+    names = json.loads(res.stdout.splitlines()[-1])
+    if not all(any("fbbev::" in n for n in case) for case in names):
+        pytest.skip("the profiler reported no library kernel")
+    ran = [any(KERNEL in n for n in case) for case in names]
+    assert ran == [True, True, False, False, False, False], ran
 
 
 def test_bench_workload_tensors():
