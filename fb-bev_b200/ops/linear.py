@@ -20,20 +20,76 @@ MAX_N = 192  # widest column block of one launch
 # in both layouts (the backward kernels' operands)
 _CACHE_ATTRS = ("_fbbev_packed", "_fbbev_packed_ffn", "_fbbev_packed_t",
                 "_fbbev_packed_ffn_t")
+# set on a tensor that a training step captured into a CUDA graph reads: the
+# graph's replays (its optimizer step) may change it in place without moving
+# its version counter, so no cache keyed on that counter holds anything derived
+# from it from then on
+_GRAPHED_ATTR = "_fbbev_graph_trained"
 
 
-def _pack(weight, transpose=False):
+def mark_graph_trained(*tensors):
+    """Mark parameters read by a training step under CUDA-graph capture and
+    drop the images cached on them.  From then on no cache keyed on their
+    version counters (the packed images here, :func:`linear_pair`'s
+    concatenation, ``CustormLearnedPositionalEncoding``'s encoding) holds
+    anything derived from them, so eager and inference calls after replays
+    see their current values."""
+    for t in tensors:
+        if t is None:
+            continue
+        for a in _CACHE_ATTRS:
+            if hasattr(t, a):
+                delattr(t, a)
+        try:
+            setattr(t, _GRAPHED_ATTR, True)
+        except AttributeError:  # a tensor type without a __dict__
+            pass
+
+
+def graph_trained(*tensors):
+    """True when one of ``tensors`` was marked by :func:`mark_graph_trained`."""
+    return any(t is not None and getattr(t, _GRAPHED_ATTR, False)
+               for t in tensors)
+
+
+def _cached(weight, attr, key, train):
+    """The cached image ``attr`` of ``weight`` under ``key``, or None; decides
+    whether the caller may cache the image it builds (returns ``(hit, may)``).
+
+    A training call (``train``) captured into a CUDA graph records its pack
+    launch: the graph then re-forms the image from the weight's storage on
+    every replay, so in-place weight updates between or inside replays
+    (optimizer steps) are honoured.  Such a call neither reads nor writes the
+    cache -- a hit would bake the capture-time weights into the graph, and an
+    image allocated from the graph's pool would be overwritten by replays --
+    and it marks the weight so that no later call caches its image either.
+    Inference captures (grad disabled) keep the cache: their graph treats the
+    weights as constants (see :func:`invalidate`)."""
+    if train and torch.cuda.is_current_stream_capturing():
+        mark_graph_trained(weight)
+        return None, False
+    if graph_trained(weight):
+        return None, False
+    hit = getattr(weight, attr, None)
+    if hit is not None and hit[0] == key:
+        return hit[1], True
+    return None, True
+
+
+def _pack(weight, transpose=False, train=False):
     """hi / lo split image of `weight` (n, k), one block per <= MAX_N columns;
     with ``transpose`` the image of ``weight.T``.
 
     Cached ON the weight tensor (so it dies with it and can never be mistaken
     for another tensor's) and keyed by storage address and version counter, so
-    an optimizer step or ``load_state_dict`` triggers a re-pack."""
+    an optimizer step or ``load_state_dict`` triggers a re-pack.  ``train``:
+    the call belongs to a training step, which never caches under CUDA-graph
+    capture (:func:`_cached`)."""
     attr = "_fbbev_packed_t" if transpose else "_fbbev_packed"
     key = (weight.data_ptr(), weight._version, tuple(weight.shape), weight.device)
-    hit = getattr(weight, attr, None)
-    if hit is not None and hit[0] == key:
-        return hit[1]
+    hit, may_cache = _cached(weight, attr, key, train)
+    if hit is not None:
+        return hit
     L = _lib.lib()
     w = weight.detach()
     w = (w.t() if transpose else w).contiguous().float()
@@ -46,10 +102,11 @@ def _pack(weight, transpose=False):
         _lib.check(L.fbbev_linear_pack(_lib.ptr(w[n0:n1]), n1 - n0, k, _lib.ptr(buf),
                                        _lib.stream_ptr(w.device)), "fbbev_linear_pack")
         blocks.append((n0, n1, buf))
-    try:
-        setattr(weight, attr, (key, blocks))
-    except AttributeError:  # a tensor type without a __dict__: no caching
-        pass
+    if may_cache:
+        try:
+            setattr(weight, attr, (key, blocks))
+        except AttributeError:  # a tensor type without a __dict__: no caching
+            pass
     return blocks
 
 
@@ -60,7 +117,13 @@ def invalidate(obj):
     The caches key on ``Tensor._version``, which in-place updates through
     ``param.data`` (EMA hooks, some checkpoint loaders) do NOT bump -- call
     this after such an update.  ``optimizer.step()``, ``load_state_dict`` and
-    ordinary in-place ops on the parameter are detected automatically."""
+    ordinary in-place ops on the parameter are detected automatically.
+
+    A CUDA graph captured with gradients off (inference) reads the images the
+    capture found and treats the weights as constants: after
+    ``load_state_dict`` or any other weight change, call this and capture
+    again.  Training steps captured with autograd recording re-form the
+    images inside the graph and need neither (see :func:`_cached`)."""
     if isinstance(obj, torch.Tensor):
         for attr in _CACHE_ATTRS:
             if hasattr(obj, attr):
@@ -68,6 +131,8 @@ def invalidate(obj):
         return
     for m in obj.modules():
         m.__dict__.pop("_pair_cache", None)
+        m.__dict__.pop("_pos_cache", None)   # the learned positional encoding
+        m.__dict__.pop("_pos_tokens", None)  # and its token-major copy
         m.__dict__.pop("_fuse_cache", None)  # TemporalFusion's folded weights
         for p in m.parameters(recurse=False):
             for attr in _CACHE_ATTRS:
@@ -88,8 +153,10 @@ def supported(x, weight):
 
 
 def linear_fused(x, weight, bias=None, relu=False, residual=None, ln_weight=None,
-                 ln_bias=None, eps=1e-5):
-    """``LN(act(x @ weight.T + bias) + residual)`` with every part optional."""
+                 ln_bias=None, eps=1e-5, train=False):
+    """``LN(act(x @ weight.T + bias) + residual)`` with every part optional.
+    ``train``: the call is the forward of a training step (weight image per
+    :func:`_pack`)."""
     _lib.require_cuda(x)
     n, k = weight.shape
     assert x.shape[-1] == k
@@ -104,7 +171,7 @@ def linear_fused(x, weight, bias=None, relu=False, residual=None, ln_weight=None
         r2 = residual.reshape(-1, n)
         if r2.stride(-1) != 1 or r2.stride(0) % 4 or r2.data_ptr() % 16:
             r2 = r2.contiguous()
-    blocks = _pack(weight)
+    blocks = _pack(weight, train=train)
     if ln_weight is not None and not ln_supported(n):
         raise _lib.FbbevError("LayerNorm epilogue: n = %d does not fit" % n)
     L = _lib.lib()
@@ -139,7 +206,9 @@ def linear_pair(x, weight_a, bias_a, weight_b, bias_b, cache, x_add=None):
     input is ``x + x_add`` (``query + query_pos``), added in the kernel's loader.
 
     ``cache`` is a dict owned by the calling module; it keeps the concatenated
-    weight / bias, keyed by the parameters' storage and version counters."""
+    weight / bias, keyed by the parameters' storage and version counters, and
+    is bypassed for parameters a captured training step updates
+    (:func:`mark_graph_trained`)."""
     _lib.require_cuda(x)
     na, k = weight_a.shape
     nb = weight_b.shape[0]
@@ -149,13 +218,17 @@ def linear_pair(x, weight_a, bias_a, weight_b, bias_b, cache, x_add=None):
         return (linear_fused(x, weight_a, bias_a), linear_fused(x, weight_b, bias_b))
     key = tuple((t.data_ptr(), t._version) for t in
                 (weight_a, weight_b, bias_a, bias_b) if t is not None)
-    hit = cache.get("pair")
+    graphed = graph_trained(weight_a, weight_b, bias_a, bias_b)
+    if graphed:
+        cache.pop("pair", None)
+    hit = None if graphed else cache.get("pair")
     if hit is None or hit[0] != key:
         w = torch.cat((weight_a.detach(), weight_b.detach()), 0).float().contiguous()
         b = None if bias_a is None else torch.cat(
             (bias_a.detach(), bias_b.detach()), 0).float().contiguous()
         hit = (key, w, b)
-        cache["pair"] = hit
+        if not graphed:
+            cache["pair"] = hit
     _, w, b = hit
     lead = x.shape[:-1]
     x2 = _rows(x, k)
@@ -177,16 +250,16 @@ def linear_pair(x, weight_a, bias_a, weight_b, bias_b, cache, x_add=None):
     return ya.view(*lead, na), yb.view(*lead, nb)
 
 
-def _pack_ffn_w1(weight, transpose=False):
+def _pack_ffn_w1(weight, transpose=False, train=False):
     """W1 (hidden, embed) as hidden / 80 separately packed 80-row blocks, one
     buffer (the layout ``fbbev_ffn_fwd`` streams); with ``transpose`` the same
     layout of ``weight.T`` (W2^T for ``fbbev_ffn_bwd``).  Cached like
     :func:`_pack`."""
     attr = "_fbbev_packed_ffn_t" if transpose else "_fbbev_packed_ffn"
     key = (weight.data_ptr(), weight._version, tuple(weight.shape), weight.device)
-    hit = getattr(weight, attr, None)
-    if hit is not None and hit[0] == key:
-        return hit[1]
+    hit, may_cache = _cached(weight, attr, key, train)
+    if hit is not None:
+        return hit
     L = _lib.lib()
     w = weight.detach()
     w = (w.t() if transpose else w).contiguous().float()
@@ -198,10 +271,11 @@ def _pack_ffn_w1(weight, transpose=False):
         _lib.check(L.fbbev_linear_pack(
             _lib.ptr(w[80 * c:80 * c + 80]), 80, k, _lib.ptr(buf[per * c:]),
             _lib.stream_ptr(w.device)), "fbbev_linear_pack")
-    try:
-        setattr(weight, attr, (key, buf))
-    except AttributeError:
-        pass
+    if may_cache:
+        try:
+            setattr(weight, attr, (key, buf))
+        except AttributeError:
+            pass
     return buf
 
 
@@ -256,7 +330,8 @@ class LinearTF32Function(torch.autograd.Function):
         y = linear_fused(
             x.detach(), weight.detach(),
             None if bias is None else bias.detach(), relu=relu,
-            residual=None if residual is None else residual.detach())
+            residual=None if residual is None else residual.detach(),
+            train=True)
         ctx.relu = relu
         ctx.has_bias = bias is not None
         ctx.has_res = residual is not None
@@ -354,7 +429,7 @@ class LinearLNTrainFunction(torch.autograd.Function):
         y = torch.empty((m, n), dtype=torch.float32, device=dev)
         xhat = torch.empty((m, n), dtype=torch.float32, device=dev)
         rstd = torch.empty((m,), dtype=torch.float32, device=dev)
-        (_, _, buf), = _pack(weight)
+        (_, _, buf), = _pack(weight, train=True)
         _lib.check(_lib.lib().fbbev_linear_fwd_ln_train(
             _lib.ptr(x2), x2.stride(0), _lib.ptr(buf),
             _lib.ptr(bias.detach().contiguous()) if bias is not None else None,
@@ -376,7 +451,7 @@ class LinearLNTrainFunction(torch.autograd.Function):
         gx = gw = gb = gr = None
         if ctx.needs_input_grad[0]:
             gx = torch.empty((dz.shape[0], k), dtype=torch.float32, device=dz.device)
-            _run_blocks(dz, _pack(weight, transpose=True), n, gx)
+            _run_blocks(dz, _pack(weight, transpose=True, train=True), n, gx)
             gx = gx.view(ctx.x_shape)
         if ctx.needs_input_grad[1]:
             gw = dz.t() @ x2
@@ -435,9 +510,9 @@ class FFNTrainFunction(torch.autograd.Function):
         if ln_weight is not None:
             xhat = torch.empty((m, embed), dtype=torch.float32, device=dev)
             rstd = torch.empty((m,), dtype=torch.float32, device=dev)
-        (_, _, w2p), = _pack(w2)
+        (_, _, w2p), = _pack(w2, train=True)
         _lib.check(_lib.lib().fbbev_ffn_fwd_train(
-            _lib.ptr(x2), x2.stride(0), _lib.ptr(_pack_ffn_w1(w1)),
+            _lib.ptr(x2), x2.stride(0), _lib.ptr(_pack_ffn_w1(w1, train=True)),
             _lib.ptr(b1.detach().contiguous()) if b1 is not None else None,
             _lib.ptr(w2p),
             _lib.ptr(b2.detach().contiguous()) if b2 is not None else None,
@@ -467,10 +542,10 @@ class FFNTrainFunction(torch.autograd.Function):
         m = dz.shape[0]
         dh = torch.empty_like(act)
         dx = torch.empty((m, embed), dtype=torch.float32, device=dz.device)
-        (_, _, w1tp), = _pack(w1, transpose=True)
+        (_, _, w1tp), = _pack(w1, transpose=True, train=True)
         _lib.check(_lib.lib().fbbev_ffn_bwd(
             _lib.ptr(dz), dz.stride(0), _lib.ptr(act),
-            _lib.ptr(_pack_ffn_w1(w2, transpose=True)), _lib.ptr(w1tp),
+            _lib.ptr(_pack_ffn_w1(w2, transpose=True, train=True)), _lib.ptr(w1tp),
             int(ctx.res == 1), m, embed, hidden, _lib.ptr(dh), _lib.ptr(dx),
             dx.stride(0), _lib.stream_ptr(dz.device)), "fbbev_ffn_bwd")
         need = ctx.needs_input_grad

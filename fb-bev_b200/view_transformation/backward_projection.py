@@ -96,10 +96,20 @@ def _fused_linear_on(x, *dropouts):
     return True
 
 
+def _note_capture(*params):
+    """Under CUDA-graph capture with autograd recording, mark ``params`` as
+    updated by the captured step (``ops.linear.mark_graph_trained``): the
+    inference caches derived from them are bypassed from then on."""
+    if (torch.is_grad_enabled() and params[0].is_cuda and
+            torch.cuda.is_current_stream_capturing()):
+        _linear_ops.mark_graph_trained(*params)
+
+
 def _linear(mod, x, relu=False, residual=None, norm=None):
     """``norm(act(mod(x)) + residual)`` in one kernel launch per <= 160 output
     columns (``mod`` an nn.Linear, ``norm`` an nn.LayerNorm or None)."""
     n, k = mod.weight.shape
+    _note_capture(mod.weight, mod.bias)
     if k % 4 or n % 4:
         y = mod(x)
         y = F.relu(y) if relu else y
@@ -189,9 +199,14 @@ class CustormLearnedPositionalEncoding(BaseModule):
     def forward(self, bs, h, w, device):
         # with gradients off the encoding is a constant of the two embedding
         # tables: build it once per (shape, table version) instead of ~8
-        # gather / repeat / cat kernels every forward
+        # gather / repeat / cat kernels every forward -- except for tables a
+        # captured training step updates (its replays move no version counter)
         key = None
-        if not torch.is_grad_enabled():
+        tables = (self.col_embed.weight, self.row_embed.weight)
+        _note_capture(*tables)
+        if _linear_ops.graph_trained(*tables):
+            self.__dict__.pop('_pos_cache', None)
+        elif not torch.is_grad_enabled():
             key = (bs, h, w, str(device), self.col_embed.weight._version,
                    self.row_embed.weight._version,
                    self.col_embed.weight.data_ptr(),
